@@ -1,13 +1,15 @@
 #!/usr/bin/env python
-"""bench.py — denoise-step throughput of the StreamingSVD hot path on B200 (BASELINE.json metric).
+"""bench.py — denoise-step throughput of the StreamingSVD hot path on H100 (BASELINE.json metric).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
 
 A "step" = ONE pass of the hot path over one batch: StreamingWrapper.forward (ControlNet on 2x7 frames + VideoUNet
 with 13 CAM mergers on 2x25 frames, 576x1024 -> latent 72x128, classifier-free-guidance batch 2) followed by the
 denoiser scalings, guider combine and Euler update of the sampler (denoiser.py:33-39, guiders.py:78-86,
 sampling.py:100-103; two fused elementwise kernels, streamingt2v_b200/sampler.py) — the work of one of
 the 150 autoregressive denoise steps of a 200-frame request (SURVEY.md §3.2).  181.96 TFLOP algorithmic.
+--dump-outputs DIR writes the latent the last timed step returned as DIR/latent.npy (float32, 3.7 MB); inputs and
+weights are seeded, so two builds can be compared output for output.
 Weights are random-init of the shipped architecture (no checkpoints offline), inputs synthetic; bf16 compute.
 
 Timed region (per rank): [invalidate conditioning cache] K x forward(+sampler math), bracketed by barrier +
@@ -20,7 +22,7 @@ is once per 30-step chunk in the real pipeline.
            memory and the result copied back to the host EVERY step; conditioning uploaded from the host once
            inside the timed region (it is constant over a chunk).
   roofline / cpu_baseline: see DESIGN.md §measurement.
-  gpu_reference : the reference's own computation as eager PyTorch on the SAME B200 — the oracle port (functional
+  gpu_reference : the reference's own computation as eager PyTorch on the SAME GPU — the oracle port (functional
            restatement of StreamingWrapper.forward, pinned against the unmodified reference) under fp16 autocast
            with cuDNN / cuBLAS / flash-SDPA, same inputs and weights, CUDA-event timed, own clocks record.  A
            reported baseline ("are we faster than torch + libraries on this box?"), never the product path.
@@ -39,6 +41,8 @@ import subprocess
 import sys
 import threading
 import time
+
+import numpy as np
 
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
@@ -61,7 +65,7 @@ def _workload(args):
     return dict(workload="StreamingSVD denoise step (ControlNet+VideoUNet+CAM), 25 frames, 576x1024 (latent 72x128), "
                          "CFG batch 2 — BASELINE configs[1]/[2] per-step unit",
                 frames=25, latent=[72, 128], cfg_batch=2, cam=True, step_tflop=STEP_TFLOP,
-                l2="inputs larger than L2 (activations ~19 GB/step >> 126 MB)", parallelism=_parallelism(args))
+                l2="inputs larger than L2 (activations ~19 GB/step >> 50 MB)", parallelism=_parallelism(args))
 
 
 # ----------------------------------------------------------------------------------------------------------------
@@ -297,7 +301,7 @@ def run_ours(args):
     rank = int(os.environ.get("RANK", "0"))
     local = int(os.environ.get("LOCAL_RANK", "0"))
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py needs a CUDA device (B200); there is no CPU path for the product arm")
+        raise SystemExit("bench.py needs a CUDA device (H100); there is no CPU path for the product arm")
     torch.cuda.set_device(local)
     dev = torch.device("cuda", local)
     pair_mode = world > 1 and args.mode == "latency"
@@ -387,10 +391,9 @@ def run_ours(args):
     cur = xd[T:2 * T].clone()
     for i in range(args.warmup):
         cur = step(cur, td, cd, ctrl_d, i)
-    # clock settling: the B200 runs this workload at its power cap (sw_power_cap, ~1.5-1.7 of 1.965 GHz); for the first
-    # seconds of sustained load the governor overshoots and then over-throttles, which made the first timed leg up to
-    # 6 % slower than the second on the same box (profiles/r02_bench_7*.json).  Extra UNTIMED steps until the load has
-    # lasted about `--settle` seconds; the timed region is still exactly K steps.
+    # clock settling: a power-capped GPU lowers its clocks during the first seconds of sustained load, which makes the
+    # first timed leg slower than later ones.  Extra UNTIMED steps until the load has lasted about `--settle` seconds;
+    # the timed region is still exactly K steps.
     settle_steps = int(round(args.settle * 5))     # a fixed count (~0.2 s per step): every rank runs the same collectives
     for _ in range(settle_steps):
         cur = step(cur, td, cd, ctrl_d, max(args.warmup - 1, 0))
@@ -411,6 +414,9 @@ def run_ours(args):
     launches = ops.launches() - l0
     ms = e0.elapsed_time(e1)
     finite = bool(torch.isfinite(cur).all())
+    if args.dump_outputs and rank == 0:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "latent.npy"), cur.float().cpu().numpy())
 
     # ---------------- e2e leg: host buffers, H2D + D2H every step ----------------
     out_host = torch.empty((T, 4, h, w), dtype=torch.float32).pin_memory()
@@ -495,27 +501,17 @@ def run_ours(args):
             peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         except Exception:
             pass
-        peak = float(peaks.get("bf16_tflops_sustained", 1400.0))
-        which = "measured (MEASURED_PEAKS.json bf16_tflops_sustained)" if peaks else "fallback 1.4 PFLOP/s sustained"
+        # NVIDIA H100 SXM data sheet (700 W card): 989 TFLOP/s dense BF16, 3.35 TB/s HBM3; a power-limited card reaches less
+        peak = float(peaks.get("bf16_tflops_sustained", 989.0))
+        which = ("measured (MEASURED_PEAKS.json bf16_tflops_sustained)" if peaks else
+                 "H100 SXM data sheet, dense BF16 (not a measured rate)")
         g = prof.families["mtgemm"]
         ach = g["flops"] / (g["ms"] * 1e-3) / 1e12
-        roof = {"kernel": "mtgemm_kernel (tcgen05 multi-tap GEMM: all Linear / Conv2d / Conv3d)", "bound": "tensor",
+        roof = {"kernel": "mtgemm_kernel (wgmma multi-tap GEMM: all Linear / Conv2d / Conv3d)", "bound": "tensor",
                 "achieved": ach, "peak": peak, "unit": "TFLOP/s", "frac": ach / peak, "peak_source": which,
                 "launches": g["launches"], "avg_launch_ms": g["ms"] / g["launches"],
-                "share_of_step": g["ms"] / sum(v["ms"] for v in prof.families.values()),
-                "traffic": None, "traffic_note": "see profiles/ for the ncu --set full capture of this kernel"}
-        try:
-            tpath = os.path.join(ROOT, "profiles", "r02_ncu_traffic.json")
-            if not os.path.exists(tpath):
-                tpath = os.path.join(ROOT, "profiles", "r01_ncu_traffic.json")
-            tr = json.load(open(tpath))["mtgemm_conv3x3_L0_320to320"]
-            roof["traffic"] = tr["traffic_bytes"]
-            roof["traffic_note"] = (f"ncu --set full, one launch of the dominant conv shape ({tr['launch']}): "
-                                    f"{tr['traffic_bytes'] / 1e6:.0f} MB DRAM vs {tr['algorithmic_bytes'] / 1e6:.0f} MB "
-                                    f"algorithmic; roofline.achieved aggregates all {g['launches']} launches of the step")
-        except Exception:
-            pass
-        hbm_peak = float(peaks.get("hbm_gbs", 6500.0))
+                "share_of_step": g["ms"] / sum(v["ms"] for v in prof.families.values())}
+        hbm_peak = float(peaks.get("hbm_gbs", 3350.0))
         for k, v in fam.items():
             if v["tflops"] > 0 and v["ms"] > 0:
                 v["tflops_per_s"] = round(v["tflops"] / (v["ms"] * 1e-3), 1)
@@ -663,6 +659,8 @@ def main():
     ap.add_argument("--no-gpu-reference", action="store_true")
     ap.add_argument("--no-chunk", action="store_true")
     ap.add_argument("--no-replicas-leg", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the latent returned by the last timed step to DIR/latent.npy (float32)")
     ap.add_argument("--mode", default="latency", choices=["latency", "throughput"],
                     help="N>1 only: latency = guidance halves on rank pairs (default), throughput = N replicas")
     args = ap.parse_args()
@@ -675,7 +673,8 @@ def main():
         cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", f"--nproc-per-node={args.gpus}",
                "--master-addr", "127.0.0.1", "--master-port", os.environ.get("MASTER_PORT", "29511"),
                os.path.abspath(__file__), "--gpus", str(args.gpus), "--steps", str(args.steps), "--warmup",
-               str(args.warmup), "--mode", args.mode] + (["--no-cpu-baseline"] if args.no_cpu_baseline else [])
+               str(args.warmup), "--mode", args.mode] + (["--no-cpu-baseline"] if args.no_cpu_baseline else []) + (
+                   ["--dump-outputs", args.dump_outputs] if args.dump_outputs else [])
         raise SystemExit(subprocess.call(cmd))
     run_ours(args)
 

@@ -1,4 +1,4 @@
-/* b200svd — C ABI of the B200-native StreamingSVD denoiser kernels (libb200svd.so).
+/* b200svd — C ABI of the H100-native (sm_90a) StreamingSVD denoiser kernels (libb200svd.so).
  *
  * The reference (Picsart-AI-Research/StreamingT2V, pure Python) has no FFI: its seam for this path is the
  * nn.Module call `StreamingWrapper.forward(x, t, c, **kwargs)` (code/models/diffusion/wrappers.py:23-78).  Every
@@ -12,7 +12,7 @@
  *   - every function enqueues work on `stream` and returns without synchronising.
  *   - return value 0 = success; non-zero = failure, message via b200svd_last_error() (thread local).
  *   - activations are bf16, channel-last: [frames, H, W, C] == [(b t), (h w), c] token rows.
- *   - no CPU fallback, no backend dispatch: sm_100a only.
+ *   - no CPU fallback, no backend dispatch: sm_90a only.
  */
 #ifndef B200SVD_H
 #define B200SVD_H
@@ -31,10 +31,10 @@ enum { B200SVD_ACT_NONE = 0, B200SVD_ACT_SILU = 1, B200SVD_ACT_GELU = 2, B200SVD
 /* ---- library ------------------------------------------------------------------------------------------- */
 const char* b200svd_last_error(void);
 int b200svd_version(void);
-/* 0 if the current device is sm_100 and the driver entry points resolve, else error. */
+/* 0 if the current device is sm_90 and the driver entry points resolve, else error. */
 int b200svd_init(int device);
 
-/* ---- multi-tap tensor-core GEMM (tcgen05 + TMEM + TMA) --------------------------------------------------
+/* ---- multi-tap tensor-core GEMM (wgmma + TMA) ------------------------------------------------------------
  * out[row, n] = s_acc * act( sum_{tap, k} A_tap[row, k] * W[tap, n, k] + bias[n] + fvec[row / rows_per_frame, n] )
  *               + s1 * res1[row, n] + s2 * res2[row, n]
  *
@@ -42,7 +42,7 @@ int b200svd_init(int device);
  * 3x3 Conv2d stride 1/2 (openaimodel.py:107-207, 257-305), (3,1,1) Conv3d of the time_stack
  * (video_model.py:46-59) — the A operand is addressed through a rank-5 TMA view of the channel-last activation,
  * each tap is a coordinate offset in that view (out-of-bounds = zero padding), and all taps accumulate into one
- * TMEM accumulator.  The epilogue carries the reference's elementwise neighbours: bias, per-frame embedding add
+ * register accumulator.  The epilogue carries the reference's elementwise neighbours: bias, per-frame embedding add
  * (openaimodel.py:346-352), GEGLU (attention.py:94-101), residual adds and AlphaBlender (util.py:358-370).
  */
 typedef struct {
@@ -93,22 +93,19 @@ typedef struct {
 
 int b200svd_gemm(const b200svd_gemm_params* p, void* stream);
 
-/* Tuning knob (no reference counterpart): when the 160/256-wide tiles run as 2-SM (tcgen05 cta_group::2, CTA-pair)
- * tiles.  0 = never, 2 = automatic (the default: every launch with at least two M tiles; also settable through the
- * environment variable B200SVD_PAIR), 1 = as 2 plus the 128-wide tile.  Other values only query.  Returns the
- * previous mode. */
+/* Kept for ABI compatibility (no reference counterpart): records a CTA-pair tile mode 0..3 and returns the previous
+ * one.  sm_90 has no CTA-pair MMA; every launch uses single-CTA tiles whatever the mode.  Other values only query. */
 int b200svd_gemm_pair_mode(int mode);
 
-/* ---- FlashAttention forward, head dim 64 (tcgen05 + TMEM + TMA) -------------------------------------------
+/* ---- FlashAttention forward, head dim 64 (wgmma + TMA) -----------------------------------------------------
  * Spatial self-attention core of BasicTransformerBlock.attn1 (attention.py:320-351 SDPA / :427-446 xformers).
  * qkv: [(n s), ldqkv] bf16, columns [q | k | v] each heads*64 wide (output of the fused QKV projection);
  * out: [(n s), ldo] bf16.  softmax(q k^T * scale) v per (frame, head). */
 int b200svd_flash_attn(const void* qkv, int64_t ldqkv, void* out, int64_t ldo, int n, int s, int heads, float scale,
                        void* stream);
 
-/* Tuning knob (no reference counterpart): softmax organisation of b200svd_flash_attn.  3 = two passes over the scores
- * (block max, then exp), 4 = one optimistic pass (default), 5 = sixteen softmax warps (each query row split over two
- * threads).  All three are parity-tested; other values only query.  Returns the previous variant. */
+/* Kept for ABI compatibility (no reference counterpart): records a softmax variant 3..5 and returns the previous one.
+ * The sm_90 kernel has a single softmax organisation whatever the variant.  Other values only query. */
 int b200svd_flash_attn_variant(int v);
 
 /* ---- small-sequence attention, head dim 64, one warp per (batch, pixel, head) -----------------------------
@@ -120,10 +117,10 @@ int b200svd_small_attn(const void* q, int64_t ldq, const void* k, int64_t ldk, c
                        int64_t ldo, int b, int s_pixels, int heads, int lq, int lk, int kv_per_pixel, float scale,
                        void* stream);
 
-/* ---- per-pixel attention over frames on the tensor cores (tcgen05), head dim 64, K/V per pixel ------------
+/* ---- per-pixel attention over frames on the tensor cores (wgmma), head dim 64, K/V per pixel ------------
  * Same contract as b200svd_small_attn with kv_per_pixel = 1: temporal self-attention (video_attention.py:145-148)
  * and CAM cross-frame attention (cam/conditioning.py:65-68).  One CTA = 4 pixels x 1 head; frames are gathered by
- * TMA through their row stride, scores are block-diagonal in a 128 x 128 tcgen05 tile. */
+ * TMA through their row stride, scores are block-diagonal in a 64 x 64 wgmma tile per two pixels. */
 int b200svd_pixel_attn(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv, void* o,
                        int64_t ldo, int b, int s_pixels, int heads, int lq, int lk, float scale, void* stream);
 

@@ -57,6 +57,9 @@ def check_grammar(wrapper, cfg):
         print(f"  grammar {name}: {len(ref)} tensors, {sum(int(np.prod(s)) for s in ref.values()) / 1e6:.1f} M params OK")
 
 
+FIXTURE_STRIDES = {"tiny_t7_24x40": (2, 1), "full_t8_64x64": (32, 2)}
+
+
 def run_case(name, cfg, T, h, w, ctx_tokens, seed):
     print(f"[{name}] building reference modules ...", flush=True)
     torch.manual_seed(0)
@@ -92,11 +95,13 @@ def run_case(name, cfg, T, h, w, ctx_tokens, seed):
     scale = ref_out.abs().max().item()
     assert err <= 2e-4 * max(scale, 1.0), f"oracle restatement deviates from the reference: {err}"
     os.makedirs(GOLDEN, exist_ok=True)
-    cstep = 8 if name.startswith("full") else 1
+    # fixture size (each file stays under 1 MB): the larger cases keep every cstep-th channel of the ControlNet taps
+    # and every hstep-th latent row of the output; the tests slice likewise
+    cstep, hstep = FIXTURE_STRIDES.get(name, (8 if name.startswith("full") else 1, 1))
     np.savez_compressed(
         os.path.join(GOLDEN, f"streaming_{name}.npz"),
-        out=ref_out.numpy().astype(np.float32),
-        # full-width cases keep every 8th channel of the ControlNet taps (fixture size); the test slices likewise
+        out=ref_out[:, :, ::hstep].numpy().astype(np.float32),
+        out_hstep=np.array([hstep], np.int64),
         ctrl_mid=captured["mid"][:, ::cstep].numpy().astype(np.float32),
         ctrl_hs_last=captured["hs"][-1][:, ::cstep].numpy().astype(np.float32),
         ctrl_cstep=np.array([cstep], np.int64),

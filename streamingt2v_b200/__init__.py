@@ -1,4 +1,4 @@
-"""b200-streamingsvd: Blackwell-native (sm_100a) denoiser hot path for the StreamingSVD pipeline.
+"""b200-streamingsvd: Hopper-native (sm_90a) denoiser hot path for the StreamingSVD pipeline.
 
 Python host code over a C-ABI CUDA library (streamingt2v_b200/libb200svd.so, include/b200svd.h).
 """

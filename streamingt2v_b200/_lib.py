@@ -2,7 +2,7 @@
 
 No torch types cross this boundary: tensors are passed as raw device pointers + sizes, the CUDA stream as a
 void*.  The library is mandatory — there is no CPU or eager-PyTorch fallback; a missing/unloadable library or a
-non-Blackwell device raises.
+device other than sm_90 raises.
 """
 from __future__ import annotations
 

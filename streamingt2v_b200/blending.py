@@ -7,7 +7,7 @@ for every scheduler timestep, every chunk of `chunk_size` frames (stride `chunk_
 independently from the SAME `latents` — UNet with its own first-frame conditioning, classifier-free guidance, one
 DDIM step — and written into `latents_denoised` from a random offset inside the overlap on (offset 0 for the first
 chunk), later chunks overwriting earlier ones.  The UNet is injected: `unet(sample[2,C,cs,H,W], t, **per_chunk) ->
-[2,C,cs,H,W]` (the reference's `self.unet(...)[0]`, pipeline_i2vgen_xl.py:857-867; the B200 I2VGen-XL UNet itself is
+[2,C,cs,H,W]` (the reference's `self.unet(...)[0]`, pipeline_i2vgen_xl.py:857-867; this project's I2VGen-XL UNet itself is
 not built yet — DESIGN.md).  The guidance combine + DDIM step + blended write are ONE CUDA kernel
 (`b200svd_ddim_blend_step`); there is no CPU fallback.
 

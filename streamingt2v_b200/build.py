@@ -1,7 +1,7 @@
-"""In-tree build of libb200svd.so (hand-written sm_100a CUDA, C ABI) and of the C oracle helpers.
+"""In-tree build of libb200svd.so (hand-written sm_90a CUDA, C ABI) and of the C oracle helpers.
 
 nvcc cross-compiles without a GPU.  Objects are cached by mtime under build/ and linked into
-streamingt2v_b200/libb200svd.so, which travels to the GPU box with the repo snapshot.
+streamingt2v_b200/libb200svd.so, which is loaded from the source tree.
 """
 from __future__ import annotations
 
@@ -17,7 +17,7 @@ OBJ_DIR = ROOT / "build" / "obj"
 LIB_PATH = ROOT / "streamingt2v_b200" / "libb200svd.so"
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",
@@ -46,7 +46,7 @@ def _compile_one(src: Path, obj: Path, verbose: bool) -> None:
 
 
 def build_lib(force: bool = False, verbose: bool = False) -> Path:
-    """Compile every csrc/*.cu for sm_100a and link libb200svd.so. Returns the library path."""
+    """Compile every csrc/*.cu for sm_90a and link libb200svd.so. Returns the library path."""
     OBJ_DIR.mkdir(parents=True, exist_ok=True)
     srcs = sorted(CSRC.glob("*.cu"))
     if not srcs:
@@ -65,7 +65,7 @@ def build_lib(force: bool = False, verbose: bool = False) -> Path:
     need_link = force or bool(jobs) or not LIB_PATH.exists() or any(
         o.stat().st_mtime > LIB_PATH.stat().st_mtime for o in objs)
     if need_link:
-        cmd = [_nvcc(), "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", str(LIB_PATH),
+        cmd = [_nvcc(), "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", str(LIB_PATH),
                *[str(o) for o in objs]]
         if verbose:
             print(" ".join(cmd), flush=True)

@@ -101,7 +101,7 @@ int sm_count() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&n[slot], cudaDevAttrMultiProcessorCount, dev);
-    if (n[slot] <= 0) n[slot] = 148;
+    if (n[slot] <= 0) n[slot] = 132;
   }
   return n[slot];
 }
@@ -125,8 +125,8 @@ int b200svd_init(int device) {
   cudaDeviceProp prop;
   e = cudaGetDeviceProperties(&prop, device);
   if (e != cudaSuccess) return b200::cuda_fail(e, "cudaGetDeviceProperties");
-  if (prop.major != 10) {
-    b200::set_error("b200svd requires an sm_100-class GPU (Blackwell B200); device %d is sm_%d%d — no fallback path",
+  if (prop.major != 9 || prop.minor != 0) {
+    b200::set_error("b200svd requires an sm_90 GPU (Hopper H100); device %d is sm_%d%d — no fallback path",
                     device, prop.major, prop.minor);
     return 1;
   }

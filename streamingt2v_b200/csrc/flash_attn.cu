@@ -1,35 +1,26 @@
-// FlashAttention forward for sm_100a, head dim 64 (v2): tcgen05.mma for S = Q K^T and O += P V with all
-// accumulators in TMEM, TMA-fed Q/K/V tiles read straight from the fused QKV projection output [(n s), 3C]
-// (no head split / transpose in HBM).
+// FlashAttention forward for sm_90a, head dim 64: wgmma for S = Q K^T and O += P V with the accumulators in
+// registers, TMA-fed Q/K/V tiles read straight from the fused QKV projection output [(n s), 3C] (no head split /
+// transpose in HBM).
 //
 // Replaces the spatial self-attention core of BasicTransformerBlock.attn1
 // (reference code/models/svd/sgm/modules/attention.py:320-351 SDPA / :427-446 xformers), batch = frames,
 // heads = C/64, sequence = H*W.
 //
-// CTA = TWO 128-row query tiles (A, B) of one (frame, head); K/V blocks are loaded once per CTA and shared by both
-// tiles.  The (tile, key-block) work items t_k (k = 2*j + tile) rotate through THREE score buffers in TMEM, so the
-// QK^T MMA of item t_(k+3) is issued as soon as the PV MMA of t_k has been issued: a tile's next scores are ready
-// before its current softmax finishes (with one buffer per tile the softmax warps idled through their own
-// PV -> QK round trip and the MUFU pipe sat at 56%, profiles/r01_ncu_fa_v2_details.txt).
-//   warp 0      TMA producer (Q_A, Q_B once; K/V ring of 4 stages)
-//   warp 1      MMA issuer + TMEM owner          (warps 2, 3 idle: warpgroup 0 gives its registers away, setmaxnreg)
-//   warps 4..11 softmax: one warpgroup per query tile, one query row per thread, 224 registers per thread
-// Per 128-key block and tile:
-//   MMA : S[128x128] = Q K_j^T                       (4 x tcgen05.mma M128 N128 K16, fp32 in TMEM)
-//   SM  : one pass over the row in registers: block max, lazy running-max update, P = exp2(S*c - m*c),
-//         P written back to TMEM as packed bf16 over the S columns (no shared-memory round trip)
-//   MMA : O[128x64] += P V_j                         (8 x tcgen05.mma, A = P from TMEM, B = V MN-major from smem)
-// O stays in TMEM for the whole KV loop.  The running max is only raised when a block max exceeds it by more than
-// 2^8 (then O and l are rescaled once, by the same softmax threads); probabilities are therefore bounded by 2^8
-// instead of 1, which bf16 represents exactly as well, and the final O / l is unchanged.
+// CTA = one 128-row query tile of one (frame, head), three warpgroups:
+//   warpgroup 0      TMA producer (Q once; K/V ring of FA_KV_STAGES 128-key blocks)
+//   warpgroups 1, 2  64 query rows each.  Per key block:
+//     S[64x128] = Q K_j^T            4 x wgmma m64n128k16, both operands from shared memory
+//     online softmax in registers    row max over the quad of threads sharing a row, P = exp2(S*c - m), O and l
+//                                    rescaled when the running max rises
+//     O[64x64] += P V_j              8 x wgmma m64n64k16, A = P (bf16) from registers, B = V MN-major from smem
 #include <cuda.h>
-#include <stdlib.h>
 #include <cuda_bf16.h>
 #include <math.h>
 
 #include "../../include/b200svd.h"
 #include "common.h"
 #include "ptx.cuh"
+#include "wgmma.cuh"
 
 namespace b200 {
 
@@ -37,15 +28,10 @@ constexpr int FA_BQ = 128;
 constexpr int FA_BK = 128;
 constexpr int FA_D = 64;
 constexpr int FA_KV_STAGES = 4;
-constexpr int FA_Q_BYTES = FA_BQ * FA_D * 2;        // 16 KB per query tile
+constexpr int FA_Q_BYTES = FA_BQ * FA_D * 2;        // 16 KB
 constexpr int FA_KV_TILE_BYTES = FA_BK * FA_D * 2;  // 16 KB each for K and V
-constexpr int FA_SMEM_BYTES = 2 * FA_Q_BYTES + FA_KV_STAGES * 2 * FA_KV_TILE_BYTES + 256;
-constexpr int FA_TMEM_COLS = 512;  // score buffers [0,128) [128,256) [256,384) (P aliases the first 64 columns), O_A [384,448) O_B [448,512)
-constexpr int FA_THREADS = 12 * 32;  // warpgroup 0: TMA, MMA (+2 idle warps); warpgroups 1, 2: softmax of tile A, B
-constexpr float FA_RESCALE_THRESHOLD = 8.0f;  // log2 units
-#define B200SVD_DEFAULT_FA_V 4
-constexpr int FA_POLY_DEFAULT = 0;  // measured (tools/bench_fa.py): every 1/8 moved to the FMA pipe costs ~5%: the softmax
-                                    // warps are bound by their own dependent-latency chain, not by MUFU throughput
+constexpr int FA_SMEM_BYTES = FA_Q_BYTES + FA_KV_STAGES * 2 * FA_KV_TILE_BYTES + 256;
+constexpr int FA_THREADS = 3 * 128;
 
 struct FaParams {
   __nv_bfloat16* out;
@@ -54,642 +40,167 @@ struct FaParams {
   float scale_log2;
 };
 
-// POLY: how many of every 8 score pairs take their exp2 on the FMA pipe (ex2_poly) instead of MUFU.  The softmax
-// of a 128 x 128 tile needs 2x the MUFU time of the tile's MMAs (16 ex2/clk/SM), so the kernel is MUFU-bound.
-// FAST (v4 softmax): every key block after the first is handled in ONE pass over the scores.  The probabilities are
-// computed optimistically against the running max the row already uses while the block max is tracked on the side;
-// only if some row's block max exceeds its running max by more than 2^8 (rare after the first blocks) the block
-// falls back to the two-pass path below (rescale O and l, recompute P against the raised max).  TMEM loads are
-// software pipelined (next 32 columns in flight while the current 32 are processed), the scale/subtract and the
-// row-sum use packed FFMA2/FADD2, the max uses FMNMX3: ~3 issue slots per score instead of ~4.6, no MUFU-idle max pass.
-template <int POLY, bool FAST>
 __global__ void __launch_bounds__(FA_THREADS, 1)
 flash_attn_kernel(const __grid_constant__ CUtensorMap tmQKV, const FaParams p) {
   extern __shared__ __align__(1024) uint8_t smem[];  // SWIZZLE_128B tiles need 1024-byte alignment
   if ((smem_u32(smem) & 1023u) != 0) __trap();
-  uint8_t* sQ = smem;                      // tile X at sQ + X*16K
-  uint8_t* sKV = sQ + 2 * FA_Q_BYTES;      // stage s: K at sKV + s*32K, V at +16K
+  uint8_t* sQ = smem;
+  uint8_t* sKV = sQ + FA_Q_BYTES;  // stage s: K at sKV + s*32K, V at +16K
   uint64_t* bars = reinterpret_cast<uint64_t*>(sKV + FA_KV_STAGES * 2 * FA_KV_TILE_BYTES);
   uint64_t* q_full = bars;
-  uint64_t* kv_full = bars + 1;                       // [4]
-  uint64_t* kv_empty = kv_full + FA_KV_STAGES;        // [4]
-  uint64_t* s_full = kv_empty + FA_KV_STAGES;         // [3] per score buffer
-  uint64_t* p_full = s_full + 3;                      // [3] per score buffer
-  uint64_t* pv_done = p_full + 3;                     // [2] per tile: completes once per key block
-  uint64_t* o_done = pv_done + 2;                     // [2] per tile: completes ONCE, after the tile's last PV
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(o_done + 2);
+  uint64_t* kv_full = bars + 1;                 // [FA_KV_STAGES]
+  uint64_t* kv_empty = kv_full + FA_KV_STAGES;  // [FA_KV_STAGES]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wg = warp >> 2;
   const int head = blockIdx.y, n = blockIdx.z;
-  const int q0 = blockIdx.x * (2 * FA_BQ);
+  const int q0 = blockIdx.x * FA_BQ;
   const int nkb = (p.S + FA_BK - 1) / FA_BK;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     prefetch_tmap(&tmQKV);
     mbar_init(q_full, 1);
     for (int s = 0; s < FA_KV_STAGES; ++s) {
       mbar_init(&kv_full[s], 1);
-      mbar_init(&kv_empty[s], 1);
-    }
-    for (int bf = 0; bf < 3; ++bf) {
-      mbar_init(&s_full[bf], 1);
-      mbar_init(&p_full[bf], 4);  // one arrive per softmax warp of the tile that owns the buffer this round
-    }
-    for (int x = 0; x < 2; ++x) {
-      mbar_init(&pv_done[x], 1);
-      mbar_init(&o_done[x], 1);
+      mbar_init(&kv_empty[s], 2);  // one arrive per consumer warpgroup
     }
     fence_barrier_init();
   }
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, FA_TMEM_COLS);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  // register re-allocation between the warpgroups: the softmax rows keep 64 packed probabilities, two 32-score
-  // buffers in flight and the running statistics live (the 168-register compile-time cap spilled them)
-  if (warp < 4) {
-   asm volatile("setmaxnreg.dec.sync.aligned.u32 56;");
-   if (warp == 0) {
-    if (lane == 0) {
+  if (wg == 0) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    if (threadIdx.x == 0) {
       // ===================== TMA producer =====================
-      mbar_expect_tx(q_full, 2 * FA_Q_BYTES);
+      mbar_expect_tx(q_full, FA_Q_BYTES);
       tma_load_3d(sQ, &tmQKV, q_full, head * FA_D, q0, n);
-      tma_load_3d(sQ + FA_Q_BYTES, &tmQKV, q_full, head * FA_D, q0 + FA_BQ, n);
       for (int j = 0; j < nkb; ++j) {
         const int s = j % FA_KV_STAGES;
-        const uint32_t ph = (j / FA_KV_STAGES) & 1;
-        mbar_wait(&kv_empty[s], ph ^ 1);
+        mbar_wait_parked(&kv_empty[s], ((j / FA_KV_STAGES) & 1) ^ 1);
         uint8_t* sk = sKV + s * 2 * FA_KV_TILE_BYTES;
         mbar_expect_tx(&kv_full[s], 2 * FA_KV_TILE_BYTES);
         tma_load_3d(sk, &tmQKV, &kv_full[s], p.C + head * FA_D, j * FA_BK, n);
         tma_load_3d(sk + FA_KV_TILE_BYTES, &tmQKV, &kv_full[s], 2 * p.C + head * FA_D, j * FA_BK, n);
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      // ===================== MMA issuer =====================
-      constexpr uint32_t idesc_qk = make_idesc_f16(128, 128, 1, 0, 0);
-      constexpr uint32_t idesc_pv = make_idesc_f16(128, 64, 1, 0, 1);  // B (=V) is MN-major
-      const uint64_t qdesc[2] = {smem_desc_k_sw128(smem_u32(sQ)), smem_desc_k_sw128(smem_u32(sQ + FA_Q_BYTES))};
-      mbar_wait(q_full, 0);
-      const int nitems = 2 * nkb;  // work items t_k: key block j = k/2, tile x = k%2, score buffer k%3
-      int kv_ready = -1;           // highest key block whose K/V stage has been waited for
-      auto issue_qk = [&](int k) {
-        const int j = k >> 1, x = k & 1, bf = k % 3;
-        if (j > kv_ready) {
-          mbar_wait(&kv_full[j % FA_KV_STAGES], (j / FA_KV_STAGES) & 1);
-          tc_fence_after();
-          kv_ready = j;
-        }
-        const uint64_t kdesc = smem_desc_k_sw128(smem_u32(sKV + (j % FA_KV_STAGES) * 2 * FA_KV_TILE_BYTES));
+    return;
+  }
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+
+  // ===================== consumer warpgroups: rows 64 cw + 16 wl + rq (+ 8) of the tile =====================
+  const int cw = wg - 1, wl = warp & 3;
+  const int rq = lane >> 2, cq = lane & 3;
+  const float c = p.scale_log2;
+  const uint64_t qdesc = smem_desc_k_sw128(smem_u32(sQ + cw * (FA_Q_BYTES / 2)));
+  float o[32];
 #pragma unroll
-        for (int kk = 0; kk < 4; ++kk)
-          umma_f16_ss(tmem_base + bf * 128, qdesc[x] + kk * 2, kdesc + kk * 2, idesc_qk, kk > 0);
-        umma_commit(&s_full[bf]);
-      };
-      for (int k = 0; k < 3 && k < nitems; ++k) issue_qk(k);
-      for (int k = 0; k < nitems; ++k) {
-        const int j = k >> 1, x = k & 1, bf = k % 3;
-        const int st = j % FA_KV_STAGES;
-        // P(t_k) is in TMEM (and the scores of t_k fully consumed)
-        mbar_wait(&p_full[bf], (k / 3) & 1);
-        tc_fence_after();
-        const uint64_t vdesc = smem_desc_mn_sw128(smem_u32(sKV + st * 2 * FA_KV_TILE_BYTES + FA_KV_TILE_BYTES));
+  for (int i = 0; i < 32; ++i) o[i] = 0.f;
+  float m_run[2] = {-INFINITY, -INFINITY};  // running max, already scaled by c (log2 units)
+  float l_run[2] = {0.f, 0.f};              // this thread's part of the row sum
+  mbar_wait(q_full, 0);
+
+  for (int j = 0; j < nkb; ++j) {
+    const int st = j % FA_KV_STAGES;
+    mbar_wait(&kv_full[st], (j / FA_KV_STAGES) & 1);
+    const uint32_t sk = smem_u32(sKV + st * 2 * FA_KV_TILE_BYTES);
+    float sacc[64];
 #pragma unroll
-        for (int kk = 0; kk < 8; ++kk) {
-          // A = P from TMEM: 16 bf16 of K per MMA = 8 packed 32-bit columns; V: +2048 B (= +128 in addr>>4) per 16 keys
-          umma_f16_ts(tmem_base + 384 + x * 64, tmem_base + bf * 128 + kk * 8, vdesc + (uint64_t)(kk * 128), idesc_pv,
-                      (j > 0 || kk > 0) ? 1u : 0u);
-        }
-        umma_commit(&pv_done[x]);
-        if (j == nkb - 1) umma_commit(&o_done[x]);
-        if (x == 1) umma_commit(&kv_empty[st]);  // both tiles' QK and PV of key block j have been issued
-        // the buffer of t_k is free again once PV(t_k) has executed (tensor pipe runs in issue order)
-        if (k + 3 < nitems) issue_qk(k + 3);
-      }
+    for (int i = 0; i < 64; ++i) sacc[i] = 0.f;
+    wgmma_fence_regs(sacc);
+    wgmma_fence();
+    const uint64_t kdesc = smem_desc_k_sw128(sk);
+#pragma unroll
+    for (int kk = 0; kk < FA_D / 16; ++kk) Wgmma<128>::ss(sacc, qdesc + (uint64_t)(kk * 2), kdesc + (uint64_t)(kk * 2), 1u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(sacc);
+
+    const int kbase = j * FA_BK;
+    if (kbase + FA_BK > p.S) {  // ragged last block: keys past the sequence do not exist
+#pragma unroll
+      for (int jj = 0; jj < 16; ++jj)
+#pragma unroll
+        for (int e = 0; e < 2; ++e)
+          if (kbase + 8 * jj + 2 * cq + e >= p.S) {
+            sacc[4 * jj + e] = -INFINITY;
+            sacc[4 * jj + 2 + e] = -INFINITY;
+          }
     }
-    __syncwarp();
-   }
-  } else {
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 224;");
-    // ===================== softmax warps: tile x = (warp-4)/4, TMEM lane quadrant = warp % 4 =====================
-    const int x = (warp - 4) >> 2;
-    const int qd = warp & 3;
-    const int r = qd * 32 + lane;  // query row in tile == TMEM lane
-    const uint32_t tl = ((uint32_t)(qd * 32)) << 16;
-    const uint32_t tO = tmem_base + 384 + x * 64 + tl;
-    float m_used = -INFINITY, l_run = 0.f;
-    const float c = p.scale_log2;
-    for (int j = 0; j < nkb; ++j) {
-      const int k = 2 * j + x, bf = k % 3;
-      const uint32_t tS = tmem_base + bf * 128 + tl;
-      mbar_wait(&s_full[bf], (k / 3) & 1);
-      tc_fence_after();
-      const int kbase = j * FA_BK;
-      const bool tail = kbase + FA_BK > p.S;
-      if (FAST && j > 0 && !tail) {
-        const float mbf = m_used * c;
-        const f32x2 c2 = pack2(c, c), nmb2 = pack2(-mbf, -mbf);
-        f32x2 la = pack2(0.f, 0.f), lb = pack2(0.f, 0.f);
-        float mxa = -INFINITY, mxb = -INFINITY;
-        uint32_t pkf[64];
-        uint32_t sva[32], svb[32];
-        auto process = [&](const uint32_t (&sv)[32], const int pbase) {
+    float alpha[2];
 #pragma unroll
-          for (int i = 0; i < 16; ++i) {
-            const float s0 = __uint_as_float(sv[2 * i]), s1 = __uint_as_float(sv[2 * i + 1]);
-            if (i & 1) mxb = max3f(mxb, s0, s1);
-            else mxa = max3f(mxa, s0, s1);
-            const f32x2 x2 = fma2(pack2(s0, s1), c2, nmb2);
-            float a, b;
-            if ((i & 7) < POLY) {
-              ex2_poly2(x2, a, b);
-            } else {
-              float xa, xb;
-              unpack2(x2, xa, xb);
-              a = ex2_approx(xa);
-              b = ex2_approx(xb);
-            }
-            if (i & 1) lb = add2(lb, pack2(a, b));
-            else la = add2(la, pack2(a, b));
-            pkf[pbase + i] = pack_bf16x2(a, b);
-          }
-        };
-        {
-          tmem_ld32(tS, sva);
-          tmem_ld_wait32(sva);
-          tmem_ld32(tS + 32, svb);
-          process(sva, 0);
-          tmem_ld_wait32(svb);
-          tmem_ld32(tS + 64, sva);
-          process(svb, 16);
-          tmem_ld_wait32(sva);
-          tmem_ld32(tS + 96, svb);
-          process(sva, 32);
-          tmem_ld_wait32(svb);
-          process(svb, 48);
-        }
-        const float mxf = fmaxf(mxa, mxb);
-        const bool needf = (mxf - m_used) * c > FA_RESCALE_THRESHOLD;
-        if (!__any_sync(0xffffffffu, needf)) {
-          {
-            uint32_t t0[32], t1[32];
+    for (int h = 0; h < 2; ++h) {
+      float mx = -INFINITY;
 #pragma unroll
-            for (int i = 0; i < 32; ++i) {
-              t0[i] = pkf[i];
-              t1[i] = pkf[32 + i];
-            }
-            tmem_st32(tS + 0, t0);
-            tmem_st32(tS + 32, t1);
-          }
-          float l0, l1, l2, l3;
-          unpack2(la, l0, l1);
-          unpack2(lb, l2, l3);
-          l_run += (l0 + l1) + (l2 + l3);
-          tmem_st_wait();
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&p_full[bf]);
-          continue;
-        }
-        // rare: some row's max rose by more than the threshold -> redo this block on the two-pass path (S is intact)
-      }
-      // pass 1 over the row (TMEM reads are cheap; keeping all 128 scores live would exceed the 168-register
-      // budget that 10 warps per CTA leave per thread): block max
-      float mx0 = -INFINITY, mx1 = -INFINITY, mx2 = -INFINITY, mx3 = -INFINITY;
+      for (int jj = 0; jj < 16; ++jj) mx = fmaxf(mx, fmaxf(sacc[4 * jj + 2 * h], sacc[4 * jj + 2 * h + 1]));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+      const float m_new = fmaxf(m_run[h], mx * c);
+      alpha[h] = ex2_approx(m_run[h] - m_new);  // 0 on the first block (m_run = -inf)
+      m_run[h] = m_new;
+      float l = 0.f;
 #pragma unroll
-      for (int c0 = 0; c0 < FA_BK; c0 += 32) {
-        uint32_t sv[32];
-        tmem_ld32(tS + c0, sv);
-        tmem_ld_wait();
-        if (tail) {
+      for (int jj = 0; jj < 16; ++jj) {
 #pragma unroll
-          for (int i = 0; i < 32; ++i)
-            if (kbase + c0 + i >= p.S) sv[i] = 0xff800000u;  // -inf
-        }
-#pragma unroll
-        for (int i = 0; i < 32; i += 4) {
-          mx0 = fmaxf(mx0, __uint_as_float(sv[i]));
-          mx1 = fmaxf(mx1, __uint_as_float(sv[i + 1]));
-          mx2 = fmaxf(mx2, __uint_as_float(sv[i + 2]));
-          mx3 = fmaxf(mx3, __uint_as_float(sv[i + 3]));
+        for (int e = 0; e < 2; ++e) {
+          const float pr = ex2_approx(fmaf(sacc[4 * jj + 2 * h + e], c, -m_new));
+          sacc[4 * jj + 2 * h + e] = pr;
+          l += pr;
         }
       }
-      const float mx = fmaxf(fmaxf(mx0, mx1), fmaxf(mx2, mx3));
-      if (j == 0) {
-        m_used = mx;
-      } else {
-        const bool need = (mx - m_used) * c > FA_RESCALE_THRESHOLD;
-        if (__any_sync(0xffffffffu, need)) {
-          // rare: raise the running max and rescale O (in TMEM) and l once
-          mbar_wait(&pv_done[x], (j - 1) & 1);  // PV(j-1) has been accumulated
-          tc_fence_after();
-          const float m_new = need ? mx : m_used;
-          const float alpha = exp2f((m_used - m_new) * c);
-          uint32_t ov[32];
-#pragma unroll
-          for (int c0 = 0; c0 < FA_D; c0 += 32) {
-            tmem_ld32(tO + c0, ov);
-            tmem_ld_wait();
-#pragma unroll
-            for (int i = 0; i < 32; ++i) ov[i] = __float_as_uint(__uint_as_float(ov[i]) * alpha);
-            tmem_st32(tO + c0, ov);
-          }
-          tmem_st_wait();
-          l_run *= alpha;
-          m_used = m_new;
-        }
-      }
-      const float mb = m_used * c;
-      float l0 = 0.f, l1 = 0.f;
-      // pass 2: P = exp2(S*c - m*c), packed bf16x2, written back over the S columns (first 64 of the tile's 128).
-      // All 128 scores are read before any P column is written (P aliases S).
-      uint32_t pk[64];
-#pragma unroll
-      for (int c0 = 0; c0 < FA_BK; c0 += 32) {
-        uint32_t sv[32];
-        tmem_ld32(tS + c0, sv);
-        tmem_ld_wait();
-#pragma unroll
-        for (int i = 0; i < 16; ++i) {
-          const float xa = fmaf(__uint_as_float(sv[2 * i]), c, -mb);
-          const float xb = fmaf(__uint_as_float(sv[2 * i + 1]), c, -mb);
-          float a, b;
-          if ((i & 7) < POLY) {
-            a = ex2_poly(xa);
-            b = ex2_poly(xb);
-          } else {
-            a = ex2_approx(xa);
-            b = ex2_approx(xb);
-          }
-          if (tail) {
-            if (kbase + c0 + 2 * i >= p.S) a = 0.f;
-            if (kbase + c0 + 2 * i + 1 >= p.S) b = 0.f;
-          }
-          l0 += a;
-          l1 += b;
-          pk[(c0 >> 1) + i] = pack_bf16x2(a, b);
-        }
-      }
-      {
-        uint32_t t0[32], t1[32];
-#pragma unroll
-        for (int i = 0; i < 32; ++i) {
-          t0[i] = pk[i];
-          t1[i] = pk[32 + i];
-        }
-        tmem_st32(tS + 0, t0);
-        tmem_st32(tS + 32, t1);
-      }
-      l_run += l0 + l1;
-      tmem_st_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&p_full[bf]);
+      l_run[h] = l_run[h] * alpha[h] + l;
     }
-    // epilogue: O / l -> bf16 -> 128 B contiguous per row.  The wait is on a barrier that completes exactly once: a
-    // parity wait on pv_done is ambiguous here — a warp whose sibling is one key block behind (it took the rescale /
-    // redo path) sees the phase of block nkb-3 and would read O before the last two PV products have landed
-    mbar_wait(&o_done[x], 0);
-    tc_fence_after();
-    const int qrow = q0 + x * FA_BQ + r;
-    const float inv = 1.0f / l_run;
-    uint32_t ova[32], ovb[32];
-    tmem_ld32(tO + 0, ova);
-    tmem_ld32(tO + 32, ovb);
-    tmem_ld_wait();
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj) {
+      o[4 * jj] *= alpha[0];
+      o[4 * jj + 1] *= alpha[0];
+      o[4 * jj + 2] *= alpha[1];
+      o[4 * jj + 3] *= alpha[1];
+    }
+    // P as the A operand of m64k16: the accumulator layout of two 8-column blocks is the A fragment layout
+    uint32_t pa[8][4];
+#pragma unroll
+    for (int kk = 0; kk < 8; ++kk) {
+      pa[kk][0] = pack_bf16x2(sacc[8 * kk + 0], sacc[8 * kk + 1]);
+      pa[kk][1] = pack_bf16x2(sacc[8 * kk + 2], sacc[8 * kk + 3]);
+      pa[kk][2] = pack_bf16x2(sacc[8 * kk + 4], sacc[8 * kk + 5]);
+      pa[kk][3] = pack_bf16x2(sacc[8 * kk + 6], sacc[8 * kk + 7]);
+    }
+    const uint64_t vdesc = smem_desc_mn_sw128(sk + FA_KV_TILE_BYTES);
+    wgmma_fence_regs(o);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 8; ++kk)  // 16 keys = 16 rows of V = 2048 B (+128 in the address field)
+      Wgmma<64>::rs_tb(o, pa[kk], vdesc + (uint64_t)(kk * 128), 1u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(o);
+    if ((threadIdx.x & 127) == 0) mbar_arrive(&kv_empty[st]);
+  }
+
+  // epilogue: O / l -> bf16
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    float l = l_run[h];
+    l += __shfl_xor_sync(0xffffffffu, l, 1);
+    l += __shfl_xor_sync(0xffffffffu, l, 2);
+    const float inv = 1.0f / l;
+    const int qrow = q0 + 64 * cw + 16 * wl + rq + 8 * h;
     if (qrow < p.S) {
-      __nv_bfloat16* dst = p.out + ((int64_t)n * p.S + qrow) * p.ldo + head * FA_D;
+      __nv_bfloat16* dst = p.out + ((int64_t)n * p.S + qrow) * p.ldo + head * FA_D + 2 * cq;
 #pragma unroll
-      for (int cc = 0; cc < 4; ++cc) {
-        reinterpret_cast<uint4*>(dst)[cc] =
-            make_uint4(pack_bf16x2(__uint_as_float(ova[8 * cc]) * inv, __uint_as_float(ova[8 * cc + 1]) * inv),
-                       pack_bf16x2(__uint_as_float(ova[8 * cc + 2]) * inv, __uint_as_float(ova[8 * cc + 3]) * inv),
-                       pack_bf16x2(__uint_as_float(ova[8 * cc + 4]) * inv, __uint_as_float(ova[8 * cc + 5]) * inv),
-                       pack_bf16x2(__uint_as_float(ova[8 * cc + 6]) * inv, __uint_as_float(ova[8 * cc + 7]) * inv));
-        reinterpret_cast<uint4*>(dst)[4 + cc] =
-            make_uint4(pack_bf16x2(__uint_as_float(ovb[8 * cc]) * inv, __uint_as_float(ovb[8 * cc + 1]) * inv),
-                       pack_bf16x2(__uint_as_float(ovb[8 * cc + 2]) * inv, __uint_as_float(ovb[8 * cc + 3]) * inv),
-                       pack_bf16x2(__uint_as_float(ovb[8 * cc + 4]) * inv, __uint_as_float(ovb[8 * cc + 5]) * inv),
-                       pack_bf16x2(__uint_as_float(ovb[8 * cc + 6]) * inv, __uint_as_float(ovb[8 * cc + 7]) * inv));
-      }
+      for (int jj = 0; jj < 8; ++jj)
+        *reinterpret_cast<uint32_t*>(dst + 8 * jj) = pack_bf16x2(o[4 * jj + 2 * h] * inv, o[4 * jj + 2 * h + 1] * inv);
     }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, FA_TMEM_COLS);
   }
 }
 
-// ---------------------------------------------------------------------------------------------------------------
-// v5: SIXTEEN softmax warps.  The v3/v4 kernel is latency bound: with two softmax warps per scheduler neither the
-// MUFU pipe (70 % busy), nor the issue slots (47 %), nor the tensor pipe (31 %) saturate, fewer instructions (v4) or
-// fewer MUFU operations (exp2 on the FMA pipe) do not help.  v5 splits every query row over TWO threads (key columns
-// [0,64) and [64,128) of each block, warps w and w+4 share a TMEM lane quadrant), so that four softmax warps per
-// scheduler hide each other's TMEM / MUFU / barrier latencies.  The two halves of a row keep the same running max:
-// they exchange their block maxima through shared memory (one 64-thread named barrier per block), take the same
-// decision (commit the optimistic probabilities or redo against a raised max), keep partial row sums and rescale /
-// normalise disjoint halves of the O columns.  P of half h lives in the first 32 columns of that half's own score
-// columns (no aliasing between the halves), so the PV MMAs read their A operand from two places.
-// ---------------------------------------------------------------------------------------------------------------
-constexpr int FA5_THREADS = 20 * 32;
-constexpr int FA5_XCH_BYTES = 2 * 2 * 4 * 2 * 32 * 4;  // [parity][tile][quadrant][half][lane] floats
-constexpr int FA5_SMEM_BYTES = FA_SMEM_BYTES + FA5_XCH_BYTES;
-
-__global__ void __launch_bounds__(FA5_THREADS, 1)
-flash_attn5_kernel(const __grid_constant__ CUtensorMap tmQKV, const FaParams p) {
-  extern __shared__ __align__(1024) uint8_t smem[];
-  if ((smem_u32(smem) & 1023u) != 0) __trap();
-  uint8_t* sQ = smem;
-  uint8_t* sKV = sQ + 2 * FA_Q_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sKV + FA_KV_STAGES * 2 * FA_KV_TILE_BYTES);
-  uint64_t* q_full = bars;
-  uint64_t* kv_full = bars + 1;
-  uint64_t* kv_empty = kv_full + FA_KV_STAGES;
-  uint64_t* s_full = kv_empty + FA_KV_STAGES;
-  uint64_t* p_full = s_full + 3;
-  uint64_t* pv_done = p_full + 3;
-  uint64_t* o_done = pv_done + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(o_done + 2);
-  float* xch = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(bars) + 256);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int head = blockIdx.y, n = blockIdx.z;
-  const int q0 = blockIdx.x * (2 * FA_BQ);
-  const int nkb = (p.S + FA_BK - 1) / FA_BK;
-
-  if (warp == 0 && lane == 0) {
-    prefetch_tmap(&tmQKV);
-    mbar_init(q_full, 1);
-    for (int s = 0; s < FA_KV_STAGES; ++s) {
-      mbar_init(&kv_full[s], 1);
-      mbar_init(&kv_empty[s], 1);
-    }
-    for (int bf = 0; bf < 3; ++bf) {
-      mbar_init(&s_full[bf], 1);
-      mbar_init(&p_full[bf], 8);  // one arrive per softmax warp of the tile (4 quadrants x 2 column halves)
-    }
-    for (int x = 0; x < 2; ++x) {
-      mbar_init(&pv_done[x], 1);
-      mbar_init(&o_done[x], 1);
-    }
-    fence_barrier_init();
-  }
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, FA_TMEM_COLS);
-    tmem_relinquish();
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-
-  if (warp < 4) {
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
-    if (warp == 0) {
-      if (lane == 0) {
-        // ===================== TMA producer =====================
-        mbar_expect_tx(q_full, 2 * FA_Q_BYTES);
-        tma_load_3d(sQ, &tmQKV, q_full, head * FA_D, q0, n);
-        tma_load_3d(sQ + FA_Q_BYTES, &tmQKV, q_full, head * FA_D, q0 + FA_BQ, n);
-        for (int j = 0; j < nkb; ++j) {
-          const int s = j % FA_KV_STAGES;
-          const uint32_t ph = (j / FA_KV_STAGES) & 1;
-          mbar_wait(&kv_empty[s], ph ^ 1);
-          uint8_t* sk = sKV + s * 2 * FA_KV_TILE_BYTES;
-          mbar_expect_tx(&kv_full[s], 2 * FA_KV_TILE_BYTES);
-          tma_load_3d(sk, &tmQKV, &kv_full[s], p.C + head * FA_D, j * FA_BK, n);
-          tma_load_3d(sk + FA_KV_TILE_BYTES, &tmQKV, &kv_full[s], 2 * p.C + head * FA_D, j * FA_BK, n);
-        }
-      }
-    } else if (warp == 1) {
-      if (lane == 0) {
-        // ===================== MMA issuer (as v3/v4; P is read from two 32-column pieces) =====================
-        constexpr uint32_t idesc_qk = make_idesc_f16(128, 128, 1, 0, 0);
-        constexpr uint32_t idesc_pv = make_idesc_f16(128, 64, 1, 0, 1);
-        const uint64_t qdesc[2] = {smem_desc_k_sw128(smem_u32(sQ)), smem_desc_k_sw128(smem_u32(sQ + FA_Q_BYTES))};
-        mbar_wait(q_full, 0);
-        const int nitems = 2 * nkb;
-        int kv_ready = -1;
-        auto issue_qk = [&](int k) {
-          const int j = k >> 1, x = k & 1, bf = k % 3;
-          if (j > kv_ready) {
-            mbar_wait(&kv_full[j % FA_KV_STAGES], (j / FA_KV_STAGES) & 1);
-            tc_fence_after();
-            kv_ready = j;
-          }
-          const uint64_t kdesc = smem_desc_k_sw128(smem_u32(sKV + (j % FA_KV_STAGES) * 2 * FA_KV_TILE_BYTES));
-#pragma unroll
-          for (int kk = 0; kk < 4; ++kk)
-            umma_f16_ss(tmem_base + bf * 128, qdesc[x] + kk * 2, kdesc + kk * 2, idesc_qk, kk > 0);
-          umma_commit(&s_full[bf]);
-        };
-        for (int k = 0; k < 3 && k < nitems; ++k) issue_qk(k);
-        for (int k = 0; k < nitems; ++k) {
-          const int j = k >> 1, x = k & 1, bf = k % 3;
-          const int st = j % FA_KV_STAGES;
-          mbar_wait(&p_full[bf], (k / 3) & 1);
-          tc_fence_after();
-          const uint64_t vdesc = smem_desc_mn_sw128(smem_u32(sKV + st * 2 * FA_KV_TILE_BYTES + FA_KV_TILE_BYTES));
-#pragma unroll
-          for (int kk = 0; kk < 8; ++kk) {
-            // keys [16 kk, 16 kk + 16): 8 packed columns; half 0 at buffer columns [0,32), half 1 at [64,96)
-            const uint32_t pa = tmem_base + bf * 128 + (kk < 4 ? kk * 8 : 64 + (kk - 4) * 8);
-            umma_f16_ts(tmem_base + 384 + x * 64, pa, vdesc + (uint64_t)(kk * 128), idesc_pv, (j > 0 || kk > 0) ? 1u : 0u);
-          }
-          umma_commit(&pv_done[x]);
-          if (j == nkb - 1) umma_commit(&o_done[x]);
-          if (x == 1) umma_commit(&kv_empty[st]);
-          if (k + 3 < nitems) issue_qk(k + 3);
-        }
-      }
-      __syncwarp();
-    }
-  } else {
-    // the pool only holds what warpgroup 0 gave back: 128 x (96 - 40) = 7168 registers = 512 x 14 -> 104 per softmax thread
-    // (asking for 112 with 48 left in warpgroup 0 needed 8192 of 6144 and blocked forever: the first version hung)
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 104;");
-    // ===================== softmax warps 4..19: tile x, column half hf, TMEM lane quadrant qd =====================
-    const int e = warp - 4;
-    const int x = e >> 3;
-    const int hf = (e >> 2) & 1;
-    const int qd = warp & 3;
-    const int r = qd * 32 + lane;
-    const uint32_t tl = ((uint32_t)(qd * 32)) << 16;
-    const uint32_t tO = tmem_base + 384 + x * 64 + 32 * hf + tl;  // this thread's 32 O columns
-    const int bar_id = 1 + x * 4 + qd;
-    auto slot = [&](int par, int h) -> float* { return xch + ((((par * 2 + x) * 4 + qd) * 2 + h) * 32) + lane; };
-    float m_used = -INFINITY, l_run = 0.f;
-    const float c = p.scale_log2;
-
-    for (int j = 0; j < nkb; ++j) {
-      const int k = 2 * j + x, bf = k % 3;
-      const uint32_t tS = tmem_base + bf * 128 + 64 * hf + tl;  // my 64 score columns; P goes over the first 32
-      mbar_wait(&s_full[bf], (k / 3) & 1);
-      tc_fence_after();
-      const int kbase = j * FA_BK + 64 * hf;
-      const bool tail = j * FA_BK + FA_BK > p.S;
-      uint32_t pk[32];
-      float lsum = 0.f, rowmax;
-      bool committed = false;
-      if (j > 0 && !tail) {
-        // optimistic single pass against the running max; the block max is tracked on the side
-        const float mbf = m_used * c;
-        const f32x2 c2 = pack2(c, c), nmb2 = pack2(-mbf, -mbf);
-        f32x2 la = pack2(0.f, 0.f), lb = pack2(0.f, 0.f);
-        float mxa = -INFINITY, mxb = -INFINITY;
-#pragma unroll
-        for (int c0 = 0; c0 < 64; c0 += 32) {
-          uint32_t sv[32];
-          tmem_ld32(tS + c0, sv);
-          tmem_ld_wait();
-#pragma unroll
-          for (int i = 0; i < 16; ++i) {
-            const float s0 = __uint_as_float(sv[2 * i]), s1 = __uint_as_float(sv[2 * i + 1]);
-            if (i & 1) mxb = max3f(mxb, s0, s1);
-            else mxa = max3f(mxa, s0, s1);
-            float xa, xb;
-            unpack2(fma2(pack2(s0, s1), c2, nmb2), xa, xb);
-            const float a = ex2_approx(xa), b = ex2_approx(xb);
-            if (i & 1) lb = add2(lb, pack2(a, b));
-            else la = add2(la, pack2(a, b));
-            pk[(c0 >> 1) + i] = pack_bf16x2(a, b);
-          }
-        }
-        const float mx = fmaxf(mxa, mxb);
-        *slot(j & 1, hf) = mx;
-        named_bar_sync(bar_id, 64);
-        rowmax = fmaxf(mx, *slot(j & 1, hf ^ 1));
-        if (!__any_sync(0xffffffffu, (rowmax - m_used) * c > FA_RESCALE_THRESHOLD)) {
-          float l0, l1, l2, l3;
-          unpack2(la, l0, l1);
-          unpack2(lb, l2, l3);
-          lsum = (l0 + l1) + (l2 + l3);
-          committed = true;
-        }
-      } else {
-        // first block / ragged last block: the row max has to be known first
-        float mx = -INFINITY;
-#pragma unroll
-        for (int c0 = 0; c0 < 64; c0 += 32) {
-          uint32_t sv[32];
-          tmem_ld32(tS + c0, sv);
-          tmem_ld_wait();
-#pragma unroll
-          for (int i = 0; i < 32; ++i) {
-            float sx = __uint_as_float(sv[i]);
-            if (tail && kbase + c0 + i >= p.S) sx = -INFINITY;
-            mx = fmaxf(mx, sx);
-          }
-        }
-        *slot(j & 1, hf) = mx;
-        named_bar_sync(bar_id, 64);
-        rowmax = fmaxf(mx, *slot(j & 1, hf ^ 1));
-      }
-      if (!committed) {
-        if (j == 0) {
-          m_used = rowmax;
-        } else {
-          const bool need = (rowmax - m_used) * c > FA_RESCALE_THRESHOLD;
-          if (__any_sync(0xffffffffu, need)) {
-            // raise the running max: rescale this thread's half of the O columns and its partial row sum
-            mbar_wait(&pv_done[x], (j - 1) & 1);
-            tc_fence_after();
-            const float m_new = need ? rowmax : m_used;
-            const float alpha = exp2f((m_used - m_new) * c);
-            uint32_t ov[32];
-            tmem_ld32(tO, ov);
-            tmem_ld_wait();
-#pragma unroll
-            for (int i = 0; i < 32; ++i) ov[i] = __float_as_uint(__uint_as_float(ov[i]) * alpha);
-            tmem_st32(tO, ov);
-            tmem_st_wait();
-            l_run *= alpha;
-            m_used = m_new;
-          }
-        }
-        const float mb = m_used * c;
-        float l0 = 0.f, l1 = 0.f;
-#pragma unroll
-        for (int c0 = 0; c0 < 64; c0 += 32) {
-          uint32_t sv[32];
-          tmem_ld32(tS + c0, sv);
-          tmem_ld_wait();
-#pragma unroll
-          for (int i = 0; i < 16; ++i) {
-            float a = ex2_approx(fmaf(__uint_as_float(sv[2 * i]), c, -mb));
-            float b = ex2_approx(fmaf(__uint_as_float(sv[2 * i + 1]), c, -mb));
-            if (tail) {
-              if (kbase + c0 + 2 * i >= p.S) a = 0.f;
-              if (kbase + c0 + 2 * i + 1 >= p.S) b = 0.f;
-            }
-            l0 += a;
-            l1 += b;
-            pk[(c0 >> 1) + i] = pack_bf16x2(a, b);
-          }
-        }
-        lsum = l0 + l1;
-      }
-      tmem_st32(tS, pk);
-      l_run += lsum;
-      tmem_st_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&p_full[bf]);
-    }
-    // epilogue: row sum = the two partial sums; this thread normalises and writes 32 of the 64 output columns
-    mbar_wait(&o_done[x], 0);   // completes once, after the tile's last PV (a parity wait on pv_done is ambiguous here)
-    tc_fence_after();
-    *slot(nkb & 1, hf) = l_run;
-    named_bar_sync(bar_id, 64);
-    const float inv = 1.0f / (l_run + *slot(nkb & 1, hf ^ 1));
-    const int qrow = q0 + x * FA_BQ + r;
-    uint32_t ov[32];
-    tmem_ld32(tO, ov);
-    tmem_ld_wait();
-    if (qrow < p.S) {
-      __nv_bfloat16* dst = p.out + ((int64_t)n * p.S + qrow) * p.ldo + head * FA_D + 32 * hf;
-#pragma unroll
-      for (int cc = 0; cc < 4; ++cc) {
-        reinterpret_cast<uint4*>(dst)[cc] =
-            make_uint4(pack_bf16x2(__uint_as_float(ov[8 * cc]) * inv, __uint_as_float(ov[8 * cc + 1]) * inv),
-                       pack_bf16x2(__uint_as_float(ov[8 * cc + 2]) * inv, __uint_as_float(ov[8 * cc + 3]) * inv),
-                       pack_bf16x2(__uint_as_float(ov[8 * cc + 4]) * inv, __uint_as_float(ov[8 * cc + 5]) * inv),
-                       pack_bf16x2(__uint_as_float(ov[8 * cc + 6]) * inv, __uint_as_float(ov[8 * cc + 7]) * inv));
-      }
-    }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, FA_TMEM_COLS);
-  }
-}
-
-static int g_fa_variant = -1;  // 3 two-pass softmax, 4 single optimistic pass (default), 5 sixteen softmax warps
-static int fa_variant() {
-  if (g_fa_variant < 0) {
-    const char* fv = getenv("B200SVD_FA_V");
-    g_fa_variant = fv ? atoi(fv) : B200SVD_DEFAULT_FA_V;
-    if (g_fa_variant < 3 || g_fa_variant > 5) g_fa_variant = B200SVD_DEFAULT_FA_V;
-  }
-  return g_fa_variant;
-}
+// Kept for the C ABI: the sm_90 kernel has a single softmax organisation; the value is recorded and reported only.
+static int g_fa_variant = 4;
 
 }  // namespace b200
 
 extern "C" int b200svd_flash_attn_variant(int v) {
-  const int prev = b200::fa_variant();
+  const int prev = b200::g_fa_variant;
   if (v >= 3 && v <= 5) b200::g_fa_variant = v;
   return prev;
 }
@@ -708,32 +219,11 @@ extern "C" int b200svd_flash_attn(const void* qkv, int64_t ldqkv, void* out, int
   uint64_t strides[2] = {(uint64_t)ldqkv * 2, (uint64_t)ldqkv * 2 * (uint64_t)s};
   uint32_t box[3] = {64, 128, 1};
   if (encode_tmap_bf16(&tm, qkv, 3, dims, strides, box)) return 1;
-  // B200SVD_FA_V / b200svd_flash_attn_variant: 3 = two-pass softmax, 4 = single optimistic pass (default), 5 = sixteen
-  // softmax warps; B200SVD_FA_POLY = 0..2 of every 8 score pairs take their exp2 on the FMA pipe (measured slower,
-  // profiles/r02_bench_fa_*.txt)
-  static int poly = -1;
   static bool attr_set[B200_MAX_DEVICES] = {};
-  const int ver = fa_variant();
-  const int fast = ver == 4 ? 1 : 0, v5 = ver == 5 ? 1 : 0;
   const int slot = dev_slot();
-  if (poly < 0 || !attr_set[slot]) {
-    const char* ev = getenv("B200SVD_FA_POLY");
-    poly = ev ? atoi(ev) : FA_POLY_DEFAULT;
-    if (poly < 0 || poly > 2) poly = FA_POLY_DEFAULT;
-    cudaError_t e = cudaFuncSetAttribute(flash_attn5_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, FA5_SMEM_BYTES);
-    auto set = [&](auto kern) {
-      if (e == cudaSuccess) e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, FA_SMEM_BYTES);
-    };
-    set(flash_attn_kernel<0, false>);
-    set(flash_attn_kernel<1, false>);
-    set(flash_attn_kernel<2, false>);
-    set(flash_attn_kernel<0, true>);
-    set(flash_attn_kernel<1, true>);
-    set(flash_attn_kernel<2, true>);
-    if (e != cudaSuccess) {
-      poly = -1;
-      return cuda_fail(e, "cudaFuncSetAttribute(flash_attn)");
-    }
+  if (!attr_set[slot]) {
+    cudaError_t e = cudaFuncSetAttribute(flash_attn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, FA_SMEM_BYTES);
+    if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(flash_attn)");
     attr_set[slot] = true;
   }
   FaParams p;
@@ -743,21 +233,8 @@ extern "C" int b200svd_flash_attn(const void* qkv, int64_t ldqkv, void* out, int
   p.heads = heads;
   p.C = C;
   p.scale_log2 = scale * 1.4426950408889634f;
-  dim3 grid((s + 2 * FA_BQ - 1) / (2 * FA_BQ), heads, n);
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-#define FA_LAUNCH(P_, F_) flash_attn_kernel<P_, F_><<<grid, FA_THREADS, FA_SMEM_BYTES, st>>>(tm, p)
-  if (v5) {
-    flash_attn5_kernel<<<grid, FA5_THREADS, FA5_SMEM_BYTES, st>>>(tm, p);
-  } else if (fast) {
-    if (poly == 0) FA_LAUNCH(0, true);
-    else if (poly == 1) FA_LAUNCH(1, true);
-    else FA_LAUNCH(2, true);
-  } else {
-    if (poly == 0) FA_LAUNCH(0, false);
-    else if (poly == 1) FA_LAUNCH(1, false);
-    else FA_LAUNCH(2, false);
-  }
-#undef FA_LAUNCH
+  dim3 grid((s + FA_BQ - 1) / FA_BQ, heads, n);
+  flash_attn_kernel<<<grid, FA_THREADS, FA_SMEM_BYTES, reinterpret_cast<cudaStream_t>(stream)>>>(tm, p);
   B200_CHECK_LAUNCH("flash_attn");
   return 0;
 }

@@ -1,6 +1,6 @@
-// Multi-tap tensor-core GEMM for sm_100a (v4).
-// TMA (rank-5 activation view) -> smem (128B swizzle) -> tcgen05.mma (fp32 accumulators in TMEM, double buffered)
-// -> fused epilogue -> swizzled smem staging -> TMA store.  See include/b200svd.h for the contract.
+// Multi-tap tensor-core GEMM for sm_90a.
+// TMA (rank-5 activation view) -> smem stage ring (128B swizzle) -> wgmma (fp32 accumulators in registers)
+// -> fused epilogue from registers.  See include/b200svd.h for the contract.
 //
 // Replaces, underneath StreamingWrapper.forward (reference code/models/diffusion/wrappers.py:23-78):
 //   nn.Linear            code/models/svd/sgm/modules/attention.py:94-120,262-351, video_attention.py:23-168
@@ -9,21 +9,12 @@
 //   + their elementwise neighbours (bias, emb add openaimodel.py:346-352, GEGLU attention.py:94-101,
 //     residual / AlphaBlender diffusionmodules/util.py:358-370).
 //
-// Persistent CTAs (one per SM; CTA pairs for the 2-SM tiles) walk a contiguous run of output tiles (N tile fastest).
-// 18 warps:
-//   warp 0       TMA producer for A/B (stage ring runs ahead across tiles)
-//   warp 1       MMA issuer + TMEM owner (two accumulator buffers: tile i's epilogue overlaps tile i+1's main loop)
-//   warps 2..17  epilogue: the CTA's output is a stream of (tile, 64-column sub-tile) blocks; each warp owns one TMEM
-//                lane quadrant of every 4th block, start to finish, and never synchronises with another warp:
-//                residual block -> (TMA) -> private 4 KB staging block; TMEM -> registers -> bias / activation /
-//                residual (in place) -> 128B/64B-swizzled staging (bank-conflict free) -> one TMA store (hardware
-//                clips ragged edges).
-// 2-SM mode (template PAIR): a cluster of two CTAs computes a 256 x BN tile with tcgen05 cta_group::2 MMAs issued by
-// the leader CTA; each CTA stages its own 128 A rows and HALF of the B tile, commits are multicast to both CTAs.
-// Why (ncu, profiles/r01_ncu_gemm_*): v2 was bound by epilogue instruction issue and bank conflicts; v3's 16-column
-// per-warp work items spent >90% of issued instructions on waits and index arithmetic and kept the four warps of a
-// quadrant in lock-step through a named barrier; the large-K layers were bound by shared-memory bandwidth per FLOP,
-// which the pair tiles halve for B.
+// Persistent CTAs (one per SM) walk the output tiles with a grid stride (N tile fastest).  Three warpgroups:
+//   warpgroup 0     TMA producer for A/B (one thread; the stage ring runs ahead across tiles, so the next tile's
+//                   operands stream in while the consumers run the epilogue of the current one)
+//   warpgroups 1-2  consumers: each owns 64 rows of the 128-row tile, issues m64nBNk16 wgmma on the shared B stage
+//                   and applies the epilogue straight from its accumulator registers.
+// A convolution tap is a shifted box of the same activation view, so taps and K blocks form one reduction loop.
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <stdlib.h>
@@ -32,12 +23,7 @@
 #include "../../include/b200svd.h"
 #include "common.h"
 #include "ptx.cuh"
-
-// Defaults of the round-2 epilogue specialisations (each also has an environment switch for A/B runs).  On since the GPU
-// parity suite passed with them (tests/test_gemm_gpu.py: 216 cases; denoiser / chain / VAE goldens:
-// profiles/r02_gputest_parity_newepi.log).
-#define B200SVD_DEFAULT_LEAN_EPI 1
-#define B200SVD_DEFAULT_GEGLU_EPI 1
+#include "wgmma.cuh"
 
 namespace b200 {
 
@@ -46,8 +32,7 @@ struct GemmDev {
   uint32_t taps, kblocks;
   uint32_t n;  // GEMM N (weight rows)
   uint32_t n_tiles;
-  uint32_t total_tiles, tiles_per_cta;
-  uint32_t a_half_dim, a_half_size;  // QUAD: A-view dim whose box is halved, and the half extent
+  uint32_t total_tiles;
   uint32_t m_ext[3];
   uint32_t m_lb[3];  // log2 of box
   uint32_t m_tiles[3];
@@ -56,7 +41,6 @@ struct GemmDev {
   void* out;
   int64_t ldo;
   int32_t out_fp32;
-  int32_t tma_epi;  // 1: staged TMA-store epilogue (bf16 out), 0: direct per-row stores (fp32 out)
   const float* bias;
   const float* fvec;
   int64_t ldf;
@@ -69,7 +53,7 @@ struct GemmDev {
   const __nv_bfloat16* res2;
   int64_t ld2;
   float s2;
-  float* gn_part;           // GroupNorm partial sums of the output (EPI == 2 only), see b200svd.h
+  float* gn_part;  // GroupNorm partial sums of the output, see b200svd.h
   int32_t* gn_slot_sample;
   int64_t gn_ld;
   uint32_t gn_rows;
@@ -78,50 +62,33 @@ struct GemmDev {
 constexpr int BM = 128;
 constexpr int BK = 64;
 constexpr int A_STAGE_BYTES = BM * BK * 2;  // 16 KB
-constexpr int EPI_WARPS = 16;
-constexpr int FIRST_EPI_WARP = 2;
-constexpr int NUM_THREADS = (FIRST_EPI_WARP + EPI_WARPS) * 32;  // 576 (register cap 112 per thread)
-constexpr int OUT_BUF_BYTES = 32 * 64 * 2;   // one quadrant (32 rows) x 64 columns
+constexpr int NUM_THREADS = 3 * 128;        // producer warpgroup + two consumer warpgroups
+constexpr int SMEM_LIMIT = 232448;          // 227 KB of dynamic shared memory per block
 
-template <int BN, int CL>
+template <int BN>
 struct TileCfg {
-  static constexpr bool PAIR = CL >= 2;
-  // PAIR: two CTAs of a cluster compute a 256 x BN tile with one cta_group::2 MMA stream; each CTA stages its own
-  // 128 A rows and HALF of the B tile (the tensor cores of the pair share B), which halves B traffic per FLOP.
-  static constexpr int B_ROWS = PAIR ? BN / 2 : BN;
-  static constexpr int B_STAGE_BYTES = B_ROWS * BK * 2;
+  static constexpr int B_STAGE_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
-  // BN = 320 (pair tiles only): every layer width of the network is a multiple of 320, so there is no ragged N tile,
-  // and the tile has the fewest bytes into the SM per FLOP (36 KB per 128x320x64 MACs).  tcgen05.mma takes N <= 256:
-  // two MMAs of N = 160 per k step, each CTA stages two 80-row pieces of B.  320 fp32 columns fit TMEM only once, so the
-  // accumulator is single-buffered (the epilogue of tile i is exposed) — used where the main loop is long.
-  static constexpr int NMMA = (BN > 256) ? 2 : 1;
-  static constexpr int BN_MMA = BN / NMMA;
-  static constexpr int NBUF = (BN > 256) ? 1 : 2;
-  static constexpr int ACC_STRIDE = (BN <= 32) ? 32 : (BN <= 64) ? 64 : (BN <= 128) ? 128 : (BN <= 256) ? 256 : 512;
-  static constexpr int TMEM_COLS = NBUF * ACC_STRIDE;
-  static_assert(BN <= 256 || PAIR, "the 320-wide tile exists as a 2-SM tile only");
-  static constexpr int NSUB = (BN + 63) / 64;
-  static constexpr int OUT_BYTES = EPI_WARPS * OUT_BUF_BYTES;  // one private 32-row x 64-column staging block per warp
-  static constexpr int FIXED_BYTES = OUT_BYTES + 512;
-  static constexpr int STAGES_FIT = (232448 - FIXED_BYTES) / STAGE_BYTES;
+  static constexpr int GN_BYTES = 4 * BN * 8;  // per 32-row quadrant: (sum, sum of squares) per column
+  static constexpr int FIXED_BYTES = GN_BYTES + 256;
+  static constexpr int STAGES_FIT = (SMEM_LIMIT - FIXED_BYTES) / STAGE_BYTES;
   static constexpr int STAGES = STAGES_FIT > 6 ? 6 : STAGES_FIT;
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + FIXED_BYTES;
-  static_assert(STAGES >= 2, "pipeline depth");
-  static_assert(SMEM_BYTES <= 232448, "shared memory budget");
+  // accumulator registers per consumer thread: BN / 2; the 256-wide tile needs the producer's registers
+  static constexpr int CONSUMER_REGS = BN > 128 ? 232 : 160;
+  static constexpr int PRODUCER_REGS = 40;
+  static_assert(STAGES >= 3, "pipeline depth");
+  static_assert(SMEM_BYTES <= SMEM_LIMIT, "shared memory budget");
   static_assert(STAGE_BYTES % 1024 == 0, "stage alignment");
+  static_assert(2 * (STAGES + 0) * 8 <= 256 - 8, "barrier area");
 };
 
-// `tile` enumerates (N tile fastest, then M tile) — in PAIR mode (M-tile PAIR); mrank selects this CTA's M tile of the
-// pair.  An M tile index past the end decodes to coordinates beyond the extents (all rows out of bounds).
-__device__ __forceinline__ uint32_t m_tile_index(const GemmDev& p, uint32_t tile, uint32_t mmul, uint32_t mrank) {
-  return (tile / p.n_tiles) * mmul + mrank;
-}
-__device__ __forceinline__ void decode_tile(const GemmDev& p, uint32_t tile, uint32_t mmul, uint32_t mrank,
-                                            uint32_t nmul, uint32_t nrank, uint32_t& n_tile, uint32_t& mb1,
+// `tile` enumerates (N tile fastest, then M tile).  An M tile decodes to the box origin of each of the three output
+// row dimensions.
+__device__ __forceinline__ void decode_tile(const GemmDev& p, uint32_t tile, uint32_t& n_tile, uint32_t& mb1,
                                             uint32_t& mb2, uint32_t& mb3) {
-  n_tile = (tile % p.n_tiles) * nmul + nrank;  // p.n_tiles counts N work items (pairs of N tiles in QUAD mode)
-  uint32_t mt = (tile / p.n_tiles) * mmul + mrank;
+  n_tile = tile % p.n_tiles;
+  uint32_t mt = tile / p.n_tiles;
   const uint32_t t1 = mt % p.m_tiles[0];
   mt /= p.m_tiles[0];
   const uint32_t t2 = mt % p.m_tiles[1];
@@ -131,86 +98,56 @@ __device__ __forceinline__ void decode_tile(const GemmDev& p, uint32_t tile, uin
   mb3 = t3 << p.m_lb[2];
 }
 
-// EPI: 0 = generic epilogue (bias / per-frame vector / activation / two residuals, all run-time switches);
-//      1 = GEGLU with bias and nothing else (the FF1 projections, 17 % of the step): compile-time specialised, packed
-//          FFMA2 math (ptx.cuh geglu2) — the generic loop spent ~30 issue slots per output there and bound the K = 320
-//          layer at 0.45 of the tensor rate (profiles/r01_ncu_v4_geglu_details.txt).
-template <int BN, int CL, int EPI>
+__device__ __forceinline__ float ldg_bf16(const __nv_bfloat16* p) { return __bfloat162float(p[0]); }
+
+// Two adjacent bf16 elements at index i (and i + 1 if `both`): one 32-bit load when aligned.
+__device__ __forceinline__ void load_bf16_pair(const __nv_bfloat16* base, int64_t i, bool both, float& a, float& b) {
+  if (both && (i & 1) == 0) {
+    const uint32_t w = __ldg(reinterpret_cast<const unsigned int*>(base + i));
+    a = bf16_lo(w);
+    b = bf16_hi(w);
+  } else {
+    a = ldg_bf16(base + i);
+    b = both ? ldg_bf16(base + i + 1) : 0.f;
+  }
+}
+
+template <int BN>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
-mtgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmAh,
-              const __grid_constant__ CUtensorMap tmB,
-              const __grid_constant__ CUtensorMap tmO64, const __grid_constant__ CUtensorMap tmO32,
-              const __grid_constant__ CUtensorMap tmR64, const __grid_constant__ CUtensorMap tmR32, const GemmDev p) {
-  using Cfg = TileCfg<BN, CL>;
-  constexpr bool PAIR = CL >= 2;  // cta_group::2 tiles
-  constexpr bool QUAD = CL == 4;  // two pairs on the same A rows (adjacent N tiles): A halves multicast between them
+mtgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmDev p) {
+  using Cfg = TileCfg<BN>;
   constexpr int STAGES = Cfg::STAGES;
+  constexpr int R = BN / 2;  // accumulator registers per thread (m64nBN: 64 x BN over 128 threads)
   extern __shared__ __align__(1024) uint8_t smem[];  // SWIZZLE_128B operands need 1024-byte alignment
   if ((smem_u32(smem) & 1023u) != 0) __trap();
-  uint8_t* out_base = smem + STAGES * Cfg::STAGE_BYTES;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(out_base + Cfg::OUT_BYTES);
+  float* gn_x = reinterpret_cast<float*>(smem + STAGES * Cfg::STAGE_BYTES);  // [4 quadrants][BN][2]
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * Cfg::STAGE_BYTES + Cfg::GN_BYTES);
   uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* acc_full = empty_bar + STAGES;    // [2]
-  uint64_t* acc_empty = acc_full + 2;         // [2]
-  uint64_t* res_bar = acc_empty + 2;          // [EPI_WARPS] residual block landed in the warp's staging block
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(res_bar + EPI_WARPS);
-  static_assert((2 * STAGES + 4 + EPI_WARPS) * 8 + 4 <= 512, "barrier area");
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-
-  const uint32_t rank4 = PAIR ? cluster_ctarank() : 0u;
-  const uint32_t rank = rank4 & 1u;    // M tile of the pair; 0 = leader CTA (issues the MMAs)
-  const uint32_t npair = rank4 >> 1;   // QUAD: which of the two N tiles this pair computes
-  const uint32_t tile_begin = (blockIdx.x / CL) * p.tiles_per_cta;
-  const uint32_t tile_end = min(tile_begin + p.tiles_per_cta, p.total_tiles);
-  const bool geglu = (p.act == B200SVD_ACT_GEGLU);
-  const uint32_t n_out = geglu ? p.n / 2 : p.n;
-  const uint32_t tile_out_w = geglu ? (uint32_t)BN / 2 : (uint32_t)BN;  // output columns per tile
-  const uint32_t nsub_out = (tile_out_w + 63) / 64;
-  const bool use_res_ring = p.tma_epi && p.res1 != nullptr;
-
-  if (warp == 0 && lane == 0) {
-    prefetch_tmap(&tmA);
-    prefetch_tmap(&tmB);
-    if (p.tma_epi) {
-      prefetch_tmap(&tmO64);
-      prefetch_tmap(&tmO32);
-    }
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], QUAD ? 2 : 1);  // QUAD: both pairs' MMAs must have read the stage (A is shared)
-    }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(&acc_full[b], 1);
-      mbar_init(&acc_empty[b], PAIR ? 2 * EPI_WARPS : EPI_WARPS);  // one arrive per epilogue warp (of both CTAs)
-    }
-    for (int b = 0; b < EPI_WARPS; ++b) mbar_init(&res_bar[b], 1);
-    fence_barrier_init();
-  }
-  if (warp == 1) {
-    if (PAIR) {
-      tmem_alloc_2sm(tmem_slot, Cfg::TMEM_COLS);
-      tmem_relinquish_2sm();
-    } else {
-      tmem_alloc(tmem_slot, Cfg::TMEM_COLS);
-      tmem_relinquish();
-    }
-  }
-  tc_fence_before();
-  if (PAIR) cluster_sync_all();  // peer barriers are initialised before any remote arrive / multicast commit
-  else __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
+  const int wg = warp >> 2;
   const uint32_t iters_per_tile = p.taps * p.kblocks;
 
-  if (warp == 0) {
-    if (lane == 0) {
+  if (threadIdx.x == 0) {
+    prefetch_tmap(&tmA);
+    prefetch_tmap(&tmB);
+    for (int s = 0; s < STAGES; ++s) {
+      mbar_init(&full_bar[s], 1);
+      mbar_init(&empty_bar[s], 2);  // one arrive per consumer warpgroup
+    }
+    fence_barrier_init();
+  }
+  __syncthreads();
+
+  if (wg == 0) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(Cfg::PRODUCER_REGS));
+    if (threadIdx.x == 0) {
       // ===================== TMA producer (A, B) =====================
       uint32_t it = 0;
-      for (uint32_t tile = tile_begin; tile < tile_end; ++tile) {
+      for (uint32_t tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
         uint32_t n_tile, mb1, mb2, mb3;
-        decode_tile(p, tile, PAIR ? 2u : 1u, rank, QUAD ? 2u : 1u, npair, n_tile, mb1, mb2, mb3);
+        decode_tile(p, tile, n_tile, mb1, mb2, mb3);
         int base[5] = {0, 0, 0, 0, 0};
         base[p.m_adim[0]] += (int)mb1;
         base[p.m_adim[1]] += (int)mb2;
@@ -227,521 +164,190 @@ mtgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
             const uint32_t ph = (it / STAGES) & 1;
             mbar_wait_parked(&empty_bar[s], ph ^ 1);
             uint8_t* sa = smem + s * Cfg::STAGE_BYTES;
-            if (PAIR) {
-              // both CTAs' loads are credited to the leader's barrier; the leader expects the bytes of the pair
-              if (rank == 0) mbar_expect_tx(&full_bar[s], 2 * Cfg::STAGE_BYTES);
-              if (QUAD) {
-                // this CTA fetches one 64-row half of the A tile and multicasts it to itself and to its twin in the
-                // other pair (same M tile, other N tile): half the L2->SM traffic for A
-                int cc[5] = {c0 + (int)(kb * BK), c1, c2, c3, c4};
-                cc[p.a_half_dim] += (int)(npair * p.a_half_size);
-                tma_load_5d_2sm_mc(sa + npair * (A_STAGE_BYTES / 2), &tmAh, &full_bar[s], cc[0], cc[1], cc[2], cc[3],
-                                   cc[4], (uint16_t)((1u << rank) | (1u << (rank + 2))));
-              } else {
-                tma_load_5d_2sm(sa, &tmA, &full_bar[s], c0 + (int)(kb * BK), c1, c2, c3, c4);
-              }
-#pragma unroll
-              for (int hh = 0; hh < Cfg::NMMA; ++hh)
-                tma_load_3d_2sm(sa + A_STAGE_BYTES + hh * (Cfg::BN_MMA / 2) * 128, &tmB, &full_bar[s], (int)(kb * BK),
-                                n0 + hh * Cfg::BN_MMA + (int)(rank * (Cfg::BN_MMA / 2)), (int)tap);
-            } else {
-              mbar_expect_tx(&full_bar[s], Cfg::STAGE_BYTES);
-              tma_load_5d(sa, &tmA, &full_bar[s], c0 + (int)(kb * BK), c1, c2, c3, c4);
-              tma_load_3d(sa + A_STAGE_BYTES, &tmB, &full_bar[s], (int)(kb * BK), n0, (int)tap);
-            }
+            mbar_expect_tx(&full_bar[s], Cfg::STAGE_BYTES);
+            tma_load_5d(sa, &tmA, &full_bar[s], c0 + (int)(kb * BK), c1, c2, c3, c4);
+            tma_load_3d(sa + A_STAGE_BYTES, &tmB, &full_bar[s], (int)(kb * BK), n0, (int)tap);
           }
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0 && rank == 0) {
-      // ===================== MMA issuer (leader CTA only in PAIR mode) =====================
-      constexpr uint32_t idesc = make_idesc_f16(PAIR ? 2 * BM : BM, Cfg::BN_MMA, /*bf16*/ 1, 0, 0);
-      uint32_t it = 0, tcount = 0;
-      for (uint32_t tile = tile_begin; tile < tile_end; ++tile, ++tcount) {
-        const uint32_t b = Cfg::NBUF == 2 ? (tcount & 1) : 0u;
-        const uint32_t bpar = Cfg::NBUF == 2 ? ((tcount >> 1) & 1) : (tcount & 1);
-        mbar_wait_parked(&acc_empty[b], bpar ^ 1);  // epilogue has drained this accumulator buffer
-        tc_fence_after();
-        const uint32_t tacc = tmem_base + b * Cfg::ACC_STRIDE;
-        for (uint32_t i = 0; i < iters_per_tile; ++i, ++it) {
-          const uint32_t s = it % STAGES;
-          const uint32_t ph = (it / STAGES) & 1;
-          mbar_wait(&full_bar[s], ph);
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + s * Cfg::STAGE_BYTES);
-          const uint64_t adesc = smem_desc_k_sw128(sa);
-#pragma unroll
-          for (int hh = 0; hh < Cfg::NMMA; ++hh) {
-            const uint64_t bdesc = smem_desc_k_sw128(sa + A_STAGE_BYTES + hh * (PAIR ? Cfg::BN_MMA / 2 : Cfg::BN_MMA) * 128);
-            const uint32_t tacc_h = tacc + (uint32_t)(hh * Cfg::BN_MMA);
-#pragma unroll
-            for (int kk = 0; kk < BK / 16; ++kk) {
-              // advance 16 elements (32 B) along K inside the 128B swizzle atom: +2 in the (addr>>4) field
-              if (PAIR)
-                umma_f16_ss_2sm(tacc_h, adesc + (uint64_t)(kk * 2), bdesc + (uint64_t)(kk * 2), idesc, (i > 0 || kk > 0) ? 1u : 0u);
-              else
-                umma_f16_ss(tacc_h, adesc + (uint64_t)(kk * 2), bdesc + (uint64_t)(kk * 2), idesc, (i > 0 || kk > 0) ? 1u : 0u);
-            }
-          }
-          // frees the smem stage (in both CTAs of a pair) once these MMAs have read it
-          if (QUAD) umma_commit_2sm(&empty_bar[s], (uint16_t)0xF);
-          else if (PAIR) umma_commit_2sm(&empty_bar[s]);
-          else umma_commit(&empty_bar[s]);
-        }
-        // accumulator complete (signalled to the epilogue warps of both CTAs of a pair)
-        if (PAIR) umma_commit_2sm(&acc_full[b], (uint16_t)(3u << (2 * npair)));
-        else umma_commit(&acc_full[b]);
-      }
-    }
-    __syncwarp();
-  } else if (warp >= FIRST_EPI_WARP) {
-    // ===================== epilogue warps (2..17) =====================
-    // The output of the CTA is a stream of blocks (tile, 64-column sub-tile); warp (q, g) owns TMEM lane quadrant q of
-    // every block n with n % 4 == g, start to finish: residual block -> (TMA) -> private staging block; TMEM ->
-    // registers -> math (+ residual, in place) -> staging -> TMA store.  Warps never synchronise with each other, so
-    // the four warps of a scheduler hide each other's latencies.  Every warp observes acc_full and arrives on
-    // acc_empty for EVERY tile (also those it owns no block of): mbarrier parity waits are only unambiguous for a
-    // waiter that is at most one phase behind.
-    const int e = warp - FIRST_EPI_WARP;
-    const int q = warp & 3;  // TMEM lane quadrant (hardware: warp % 4)
-    const int g = e >> 2;    // block phase; warps 4g+2 .. 4g+5 cover the four quadrants once
-    const int r = q * 32 + lane;
-    const uint32_t lb1 = p.m_lb[0], lb2 = p.m_lb[1];
-    const uint32_t qoff = (uint32_t)(q * 32);
-    const uint32_t qo1 = qoff & ((1u << lb1) - 1);
-    const uint32_t qo2 = (qoff >> lb1) & ((1u << lb2) - 1);
-    const uint32_t qo3 = qoff >> (lb1 + lb2);
-    uint8_t* ob = out_base + e * OUT_BUF_BYTES;
-    uint64_t* my_res = &res_bar[e];
-    const bool bias_vec = p.bias != nullptr && (reinterpret_cast<uintptr_t>(p.bias) & 15) == 0;
-    const bool fvec_vec = p.fvec != nullptr && (reinterpret_cast<uintptr_t>(p.fvec) & 15) == 0 && (p.ldf & 3) == 0;
-    const uint32_t num_tiles = tile_end > tile_begin ? tile_end - tile_begin : 0u;
+    return;
+  }
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(Cfg::CONSUMER_REGS));
 
-    auto acc_buf = [](uint32_t t) -> uint32_t { return Cfg::NBUF == 2 ? (t & 1u) : 0u; };
-    auto acc_par = [](uint32_t t) -> uint32_t { return Cfg::NBUF == 2 ? ((t >> 1) & 1u) : (t & 1u); };
-    uint32_t tcount = 0, s = (uint32_t)g, tpass = 0, rcount = 0;
-    while (s >= nsub_out) {
-      s -= nsub_out;
-      ++tcount;
+  // ===================== consumer warpgroups =====================
+  const int cw = wg - 1;   // rows [64 cw, 64 cw + 64) of the tile
+  const int wl = warp & 3;  // warp of the warpgroup: rows 16 wl .. 16 wl + 15 of those 64
+  const int rq = lane >> 2, cq = lane & 3;
+  const bool geglu = (p.act == B200SVD_ACT_GEGLU);
+  const uint32_t n_out = geglu ? p.n / 2 : p.n;
+  const uint32_t tile_out_w = geglu ? (uint32_t)BN / 2 : (uint32_t)BN;
+  const uint32_t lb1 = p.m_lb[0], lb2 = p.m_lb[1];
+  const int quad = 2 * cw + (wl >> 1);  // 32-row quadrant of the tile
+  const bool gn = p.gn_part != nullptr;
+  const bool gn_sender = (wl & 1) != 0;
+  const int gn_bar = 1 + quad;
+  float* gxq = gn_x + quad * BN * 2;
+  uint32_t it = 0;
+  float acc[R];
+
+  for (uint32_t tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+#pragma unroll
+    for (int i = 0; i < R; ++i) acc[i] = 0.f;
+    for (uint32_t i = 0; i < iters_per_tile; ++i, ++it) {
+      const uint32_t s = it % STAGES;
+      mbar_wait(&full_bar[s], (it / STAGES) & 1);
+      const uint32_t sa = smem_u32(smem + s * Cfg::STAGE_BYTES);
+      const uint64_t adesc = smem_desc_k_sw128(sa + cw * (A_STAGE_BYTES / 2));
+      const uint64_t bdesc = smem_desc_k_sw128(sa + A_STAGE_BYTES);
+      wgmma_fence_regs(acc);
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < BK / 16; ++kk)  // +16 elements along K = +32 B inside the swizzle atom
+        Wgmma<BN>::ss(acc, adesc + (uint64_t)(kk * 2), bdesc + (uint64_t)(kk * 2), 1u);
+      wgmma_commit();
+      wgmma_fence_regs(acc);
+      // the MMAs of the previous stage have completed: hand it back to the producer
+      wgmma_wait<1>();
+      if (i > 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[(it - 1) % STAGES]);
     }
-    uint32_t n_tile = 0, mb1 = 0, mb2 = 0, mb3 = 0;
-    // residual block of (tile, s) -> staging block; the previous store must have finished reading it
-    auto prefetch_residual = [&]() {
-      const uint32_t ocol0 = n_tile * tile_out_w + 64 * s;
-      if (use_res_ring && ocol0 < n_out && lane == 0) {
-        const uint32_t rem = tile_out_w - 64 * s;
-        const uint32_t subw = rem >= 64 ? 64u : rem;
-        tma_store_wait_read<0>();
-        mbar_expect_tx(my_res, subw * 2 * 32);
-        tma_load_5d(ob, subw == 64 ? &tmR64 : &tmR32, my_res, (int)ocol0, (int)(mb1 + qo1), (int)(mb2 + qo2),
-                    (int)(mb3 + qo3), 0);
-      }
-    };
-    if (tcount < num_tiles) {
-      decode_tile(p, tile_begin + tcount, PAIR ? 2u : 1u, rank, QUAD ? 2u : 1u, npair, n_tile, mb1, mb2, mb3);
-      prefetch_residual();
-    }
-    while (tcount < num_tiles) {
-      const uint32_t n0 = n_tile * BN;
-      const uint32_t otile0 = n_tile * tile_out_w;
+    wgmma_wait<0>();
+    wgmma_fence_regs(acc);
+    if ((threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[(it - 1) % STAGES]);
+
+    // ----- epilogue: thread holds rows r0 and r0 + 8, columns 8 j + 2 cq + {0, 1} (acc[4 j + 2 h + e]) -----
+    uint32_t n_tile, mb1, mb2, mb3;
+    decode_tile(p, tile, n_tile, mb1, mb2, mb3);
+    const uint32_t n0 = n_tile * BN;
+    const uint32_t otile0 = n_tile * tile_out_w;
+    bool valid[2];
+    int64_t row[2];
+    const float* fv[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const uint32_t r = (uint32_t)(64 * cw + 16 * wl + rq + 8 * h);
       const uint32_t m1 = mb1 + (r & ((1u << lb1) - 1));
       const uint32_t m2 = mb2 + ((r >> lb1) & ((1u << lb2) - 1));
       const uint32_t m3 = mb3 + (r >> (lb1 + lb2));
-      const bool valid = (m1 < p.m_ext[0]) && (m2 < p.m_ext[1]) && (m3 < p.m_ext[2]);
-      const int64_t row = (int64_t)m1 * p.out_rs[0] + (int64_t)m2 * p.out_rs[1] + (int64_t)m3 * p.out_rs[2];
-      const float* fv = nullptr;
-      if (p.fvec != nullptr && valid) fv = p.fvec + (int64_t)((uint32_t)row / p.rows_per_frame) * p.ldf;
-      const uint32_t ocol0 = otile0 + 64 * s;
-      const bool skip = ocol0 >= n_out;  // block beyond the ragged N edge (warp-uniform)
-      const uint32_t rem = tile_out_w - 64 * s;
-      const uint32_t subw = rem >= 64 ? 64u : rem;  // 64 or 32 (direct path: also narrower tiles)
-
-      // release the accumulators of the tiles this warp owns no block of
-      for (; tpass < tcount; ++tpass) {
-        mbar_wait_parked(&acc_full[acc_buf(tpass)], acc_par(tpass));
-        if (lane == 0) {
-          if (PAIR) mbar_arrive_leader(&acc_empty[acc_buf(tpass)]);
-          else mbar_arrive(&acc_empty[acc_buf(tpass)]);
-        }
-      }
-      const uint32_t b = acc_buf(tcount);
-      mbar_wait_parked(&acc_full[b], acc_par(tcount));
-      tc_fence_after();
-      const uint32_t tlane = tmem_base + b * Cfg::ACC_STRIDE + ((uint32_t)(q * 32) << 16);
-
-      // per-16-column math shared by both epilogue flavours; v = accumulators on entry, finished values on exit
-      auto finish16 = [&](float (&v)[16], const uint32_t (&vg)[16], uint32_t wcol, uint32_t ocol, bool full) {
+      valid[h] = (m1 < p.m_ext[0]) && (m2 < p.m_ext[1]) && (m3 < p.m_ext[2]);
+      row[h] = (int64_t)m1 * p.out_rs[0] + (int64_t)m2 * p.out_rs[1] + (int64_t)m3 * p.out_rs[2];
+      fv[h] = (p.fvec != nullptr && valid[h]) ? p.fvec + (int64_t)((uint32_t)row[h] / p.rows_per_frame) * p.ldf
+                                              : nullptr;
+    }
+    constexpr int NJ = BN / 8;
+#pragma unroll
+    for (int j = 0; j < NJ; ++j) {
+      if (geglu && j >= NJ / 2) break;  // gate columns are consumed with their value columns
+      const uint32_t tcol = 8 * j + 2 * cq;  // column in the tile (value column for GEGLU)
+      const uint32_t ocol = otile0 + tcol;
+      const bool in0 = ocol < n_out, in1 = ocol + 1 < n_out;
+      float gs0 = 0.f, gs1 = 0.f, gq0 = 0.f, gq1 = 0.f;  // GroupNorm partials of the two columns
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+        if (!valid[h] || !in0) continue;
         if (p.bias != nullptr) {
-          if (full && bias_vec) {
-#pragma unroll
-            for (int j4 = 0; j4 < 4; ++j4) {
-              const float4 bb = __ldg(reinterpret_cast<const float4*>(p.bias + wcol) + j4);
-              v[4 * j4] += bb.x; v[4 * j4 + 1] += bb.y; v[4 * j4 + 2] += bb.z; v[4 * j4 + 3] += bb.w;
-            }
-          } else {
-#pragma unroll
-            for (int j = 0; j < 16; ++j)
-              if (full || ocol + j < n_out) v[j] += __ldg(p.bias + wcol + j);
-          }
+          v0 += __ldg(p.bias + n0 + tcol);
+          if (in1) v1 += __ldg(p.bias + n0 + tcol + 1);
         }
-        if (fv != nullptr) {
-          if (full && fvec_vec) {
-#pragma unroll
-            for (int j4 = 0; j4 < 4; ++j4) {
-              const float4 bb = __ldg(reinterpret_cast<const float4*>(fv + ocol) + j4);
-              v[4 * j4] += bb.x; v[4 * j4 + 1] += bb.y; v[4 * j4 + 2] += bb.z; v[4 * j4 + 3] += bb.w;
-            }
-          } else {
-#pragma unroll
-            for (int j = 0; j < 16; ++j)
-              if (full || ocol + j < n_out) v[j] += __ldg(fv + ocol + j);
-          }
+        if (fv[h] != nullptr) {
+          v0 += __ldg(fv[h] + ocol);
+          if (in1) v1 += __ldg(fv[h] + ocol + 1);
         }
         if (p.act == B200SVD_ACT_SILU) {
-#pragma unroll
-          for (int j = 0; j < 16; ++j) v[j] = silu_fast(v[j]);
+          v0 = silu_fast(v0);
+          v1 = silu_fast(v1);
         } else if (p.act == B200SVD_ACT_GELU) {
-#pragma unroll
-          for (int j = 0; j < 16; ++j) v[j] = gelu_fast(v[j]);
+          v0 = gelu_fast(v0);
+          v1 = gelu_fast(v1);
         } else if (geglu) {
-          float gt[16];
-#pragma unroll
-          for (int j = 0; j < 16; ++j) gt[j] = __uint_as_float(vg[j]);
+          float g0 = acc[4 * (j + NJ / 2) + 2 * h], g1 = acc[4 * (j + NJ / 2) + 2 * h + 1];
           if (p.bias != nullptr) {
-            if (full && bias_vec) {
-#pragma unroll
-              for (int j4 = 0; j4 < 4; ++j4) {
-                const float4 bb = __ldg(reinterpret_cast<const float4*>(p.bias + wcol + BN / 2) + j4);
-                gt[4 * j4] += bb.x; gt[4 * j4 + 1] += bb.y; gt[4 * j4 + 2] += bb.z; gt[4 * j4 + 3] += bb.w;
-              }
-            } else {
-#pragma unroll
-              for (int j = 0; j < 16; ++j)
-                if (full || ocol + j < n_out) gt[j] += __ldg(p.bias + wcol + BN / 2 + j);
-            }
+            g0 += __ldg(p.bias + n0 + BN / 2 + tcol);
+            if (in1) g1 += __ldg(p.bias + n0 + BN / 2 + tcol + 1);
           }
-#pragma unroll
-          for (int j = 0; j < 16; ++j) v[j] = v[j] * gelu_fast(gt[j]);
+          v0 *= gelu_fast(g0);
+          v1 *= gelu_fast(g1);
         }
-        if (p.s_acc != 1.0f) {
-#pragma unroll
-          for (int j = 0; j < 16; ++j) v[j] *= p.s_acc;
+        v0 *= p.s_acc;
+        v1 *= p.s_acc;
+        if (p.res1 != nullptr) {
+          float a, b;
+          load_bf16_pair(p.res1, row[h] * p.ld1 + ocol, in1, a, b);
+          v0 += p.s1 * a;
+          v1 += p.s1 * b;
         }
-      };
-
-      if (EPI == 1) {
-        if (!skip) {
-          // host guarantees: act == GEGLU, 16-byte aligned bias, no fvec / residuals, s_acc == 1, TMA-store epilogue,
-          // n % BN == 0 (every 64-column block is full)
-          if (lane == 0) tma_store_wait_read<0>();  // the previous TMA store has finished reading the staging block
-          __syncwarp();
-          uint8_t* orow = ob + lane * 128;
-          const uint32_t x = (uint32_t)(lane & 7);
-          const float4* bvp = reinterpret_cast<const float4*>(p.bias + n0 + 64 * s);
-          const float4* bgp = reinterpret_cast<const float4*>(p.bias + n0 + (uint32_t)(BN / 2) + 64 * s);
-#pragma unroll
-          for (uint32_t c = 0; c < 4; ++c) {
-            uint32_t va[16], vg[16];
-            tmem_ld16(tlane + 64 * s + 16 * c, va);
-            tmem_ld16(tlane + (uint32_t)(BN / 2) + 64 * s + 16 * c, vg);
-            tmem_ld_wait();
-            uint32_t o[8];
-#pragma unroll
-            for (int j4 = 0; j4 < 4; ++j4) {
-              const float4 bv = __ldg(bvp + 4 * c + j4);
-              const float4 bg = __ldg(bgp + 4 * c + j4);
-              const f32x2 v01 = add2(pack2u(va[4 * j4], va[4 * j4 + 1]), pack2(bv.x, bv.y));
-              const f32x2 v23 = add2(pack2u(va[4 * j4 + 2], va[4 * j4 + 3]), pack2(bv.z, bv.w));
-              const f32x2 g01 = add2(pack2u(vg[4 * j4], vg[4 * j4 + 1]), pack2(bg.x, bg.y));
-              const f32x2 g23 = add2(pack2u(vg[4 * j4 + 2], vg[4 * j4 + 3]), pack2(bg.z, bg.w));
-              float r0, r1, r2, r3;
-              unpack2(geglu2(v01, g01), r0, r1);
-              unpack2(geglu2(v23, g23), r2, r3);
-              o[2 * j4] = pack_bf16x2(r0, r1);
-              o[2 * j4 + 1] = pack_bf16x2(r2, r3);
-            }
-            *reinterpret_cast<uint4*>(orow + (((2 * c) ^ x) << 4)) = make_uint4(o[0], o[1], o[2], o[3]);
-            *reinterpret_cast<uint4*>(orow + (((2 * c + 1) ^ x) << 4)) = make_uint4(o[4], o[5], o[6], o[7]);
-          }
-          fence_proxy_async_smem();  // generic-proxy smem writes -> visible to the TMA store
+        if (p.res2 != nullptr) {
+          float a, b;
+          load_bf16_pair(p.res2, row[h] * p.ld2 + ocol, in1, a, b);
+          v0 += p.s2 * a;
+          v1 += p.s2 * b;
         }
-      } else if (EPI == 2) {
-        if (!skip) {
-          // linear family without activation: acc (+ bias) (+ per-frame vector) (* s_acc) (+ s1 res1) (+ s2 res2), all
-          // optional parts behind warp-uniform branches, arithmetic on packed pairs.  Host guarantees: TMA-store
-          // epilogue, n_out % 16 == 0 (a 16-column chunk is either complete or entirely past the edge), 16-byte
-          // aligned bias / fvec (ldf % 4 == 0).  ~4 issue slots per output instead of ~20.
-          if (use_res_ring) {
-            mbar_wait(my_res, rcount & 1);  // residual block has landed in the staging block
-            ++rcount;
+        if (p.out_fp32) {
+          float* op = reinterpret_cast<float*>(p.out) + row[h] * p.ldo + ocol;
+          if (in1 && ((row[h] * p.ldo + ocol) & 1) == 0) {
+            *reinterpret_cast<float2*>(op) = make_float2(v0, v1);
           } else {
-            if (lane == 0) tma_store_wait_read<0>();
-            __syncwarp();
+            op[0] = v0;
+            if (in1) op[1] = v1;
           }
-          uint8_t* orow;
-          uint32_t x;
-          if (subw == 64) {
-            orow = ob + lane * 128;
-            x = (uint32_t)(lane & 7);
-          } else {
-            orow = ob + lane * 64;
-            x = (uint32_t)((lane >> 1) & 3);
-          }
-          const uint32_t nchunks = subw >> 4;
-          const f32x2 s1v = splat2(p.s1), s2v = splat2(p.s2), sav = splat2(p.s_acc);
-          const bool has_res2 = p.res2 != nullptr && valid;
-#pragma unroll
-          for (uint32_t c = 0; c < 4; ++c) {
-            if (c < nchunks) {
-              const uint32_t acol = 64 * s + 16 * c;
-              const uint32_t ocol = ocol0 + 16 * c;
-              uint32_t va[16];
-              tmem_ld16(tlane + acol, va);
-              tmem_ld_wait();
-              f32x2 v[8];
-#pragma unroll
-              for (int j = 0; j < 8; ++j) v[j] = pack2u(va[2 * j], va[2 * j + 1]);
-              const bool inb = (ocol + 16) <= n_out;  // else: the whole chunk is past the N edge (TMA clips it)
-              if (p.bias != nullptr && inb) {
-                const float4* bp = reinterpret_cast<const float4*>(p.bias + n0 + acol);
-#pragma unroll
-                for (int j4 = 0; j4 < 4; ++j4) {
-                  const float4 bb = __ldg(bp + j4);
-                  v[2 * j4] = add2(v[2 * j4], pack2(bb.x, bb.y));
-                  v[2 * j4 + 1] = add2(v[2 * j4 + 1], pack2(bb.z, bb.w));
-                }
-              }
-              if (fv != nullptr && inb) {
-                const float4* fp = reinterpret_cast<const float4*>(fv + ocol);
-#pragma unroll
-                for (int j4 = 0; j4 < 4; ++j4) {
-                  const float4 bb = __ldg(fp + j4);
-                  v[2 * j4] = add2(v[2 * j4], pack2(bb.x, bb.y));
-                  v[2 * j4 + 1] = add2(v[2 * j4 + 1], pack2(bb.z, bb.w));
-                }
-              }
-              if (p.s_acc != 1.0f) {
-#pragma unroll
-                for (int j = 0; j < 8; ++j) v[j] = mul2(v[j], sav);
-              }
-              const uint32_t c_lo = 2 * c, c_hi = 2 * c + 1;
-              if (use_res_ring) {
-                const uint4 a = *reinterpret_cast<const uint4*>(orow + ((c_lo ^ x) << 4));
-                const uint4 bq = *reinterpret_cast<const uint4*>(orow + ((c_hi ^ x) << 4));
-                const uint32_t w[8] = {a.x, a.y, a.z, a.w, bq.x, bq.y, bq.z, bq.w};
-#pragma unroll
-                for (int j = 0; j < 8; ++j) v[j] = fma2(pack2(bf16_lo(w[j]), bf16_hi(w[j])), s1v, v[j]);
-              }
-              if (has_res2 && inb) {
-                const uint4* rp = reinterpret_cast<const uint4*>(p.res2 + row * p.ld2 + ocol);
-                const uint4 a = __ldg(rp);
-                const uint4 bq = __ldg(rp + 1);
-                const uint32_t w[8] = {a.x, a.y, a.z, a.w, bq.x, bq.y, bq.z, bq.w};
-#pragma unroll
-                for (int j = 0; j < 8; ++j) v[j] = fma2(pack2(bf16_lo(w[j]), bf16_hi(w[j])), s2v, v[j]);
-              }
-              uint32_t o[8];
-#pragma unroll
-              for (int j = 0; j < 8; ++j) {
-                float lo, hi;
-                unpack2(v[j], lo, hi);
-                o[j] = pack_bf16x2(lo, hi);
-              }
-              *reinterpret_cast<uint4*>(orow + ((c_lo ^ x) << 4)) = make_uint4(o[0], o[1], o[2], o[3]);
-              *reinterpret_cast<uint4*>(orow + ((c_hi ^ x) << 4)) = make_uint4(o[4], o[5], o[6], o[7]);
-              if (p.gn_part != nullptr && inb) {
-                // per-column sum / sum of squares over the 32 rows of this quadrant (of the bf16-ROUNDED values, the
-                // ones the consumer reads): 32-lane transpose-reduce, 16 + 16 shuffles; lane L ends with column
-                // (L >> 1) & 15, even lanes store 16 x (sum, sumsq) = 128 contiguous bytes
-                float a[16], b[16];
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                  const float lo = valid ? bf16_lo(o[j]) : 0.f, hi = valid ? bf16_hi(o[j]) : 0.f;
-                  a[2 * j] = lo;
-                  a[2 * j + 1] = hi;
-                  b[2 * j] = lo * lo;
-                  b[2 * j + 1] = hi * hi;
-                }
-#pragma unroll
-                for (int w = 8, bit = 16; w >= 1; w >>= 1, bit >>= 1) {
-                  const bool up = (lane & bit) != 0;
-#pragma unroll
-                  for (int i = 0; i < w; ++i) {
-                    const float keep_a = up ? a[w + i] : a[i], send_a = up ? a[i] : a[w + i];
-                    const float keep_b = up ? b[w + i] : b[i], send_b = up ? b[i] : b[w + i];
-                    a[i] = keep_a + __shfl_xor_sync(0xffffffffu, send_a, bit);
-                    b[i] = keep_b + __shfl_xor_sync(0xffffffffu, send_b, bit);
-                  }
-                }
-                a[0] += __shfl_xor_sync(0xffffffffu, a[0], 1);
-                b[0] += __shfl_xor_sync(0xffffffffu, b[0], 1);
-                if ((lane & 1) == 0) {
-                  const uint32_t slot = m_tile_index(p, tile_begin + tcount, PAIR ? 2u : 1u, rank) * 4u + (uint32_t)q;
-                  float2* dst = reinterpret_cast<float2*>(p.gn_part) + (int64_t)slot * p.gn_ld + ocol + ((lane >> 1) & 15);
-                  *dst = make_float2(a[0], b[0]);
-                }
-              }
-            }
-          }
-          if (p.gn_part != nullptr && lane == 0 && n_tile == 0 && s == 0) {
-            // lane 0 owns the first row of the quadrant: if it is out of range, so is every row of the quadrant
-            const uint32_t slot = m_tile_index(p, tile_begin + tcount, PAIR ? 2u : 1u, rank) * 4u + (uint32_t)q;
-            p.gn_slot_sample[slot] = valid ? (int32_t)((uint32_t)row / p.gn_rows) : -1;
-          }
-          fence_proxy_async_smem();
-        }
-      } else if (!skip && p.tma_epi) {
-        if (use_res_ring) {
-          mbar_wait(my_res, rcount & 1);  // residual block has landed in the staging block
-          ++rcount;
         } else {
-          if (lane == 0) tma_store_wait_read<0>();  // the previous TMA store has finished reading the staging block
-          __syncwarp();
-        }
-        uint8_t* orow;
-        uint32_t x;  // swizzle phase of this thread's staging row
-        if (subw == 64) {
-          orow = ob + lane * 128;
-          x = (uint32_t)(lane & 7);
-        } else {
-          orow = ob + lane * 64;
-          x = (uint32_t)((lane >> 1) & 3);
-        }
-        const uint32_t nchunks = subw >> 4;
-#pragma unroll 1
-        for (uint32_t c = 0; c < nchunks; ++c) {
-          const uint32_t acol = 64 * s + 16 * c;  // accumulator column (value half for GEGLU)
-          uint32_t va[16], vg[16];
-          tmem_ld16(tlane + acol, va);
-          if (geglu) tmem_ld16(tlane + (uint32_t)(BN / 2) + acol, vg);
-          tmem_ld_wait();
-          float v[16];
-#pragma unroll
-          for (int j = 0; j < 16; ++j) v[j] = __uint_as_float(va[j]);
-          const uint32_t ocol = ocol0 + 16 * c;
-          const bool full = (ocol + 16) <= n_out;
-          finish16(v, vg, n0 + acol, ocol, full);
-          const uint32_t c_lo = 2 * c, c_hi = 2 * c + 1;  // 16-byte chunks of the row
-          if (use_res_ring) {
-            // residual chunk sits where the result will go (same box, same swizzle): read, add, overwrite
-            const uint4 a = *reinterpret_cast<const uint4*>(orow + ((c_lo ^ x) << 4));
-            const uint4 bq = *reinterpret_cast<const uint4*>(orow + ((c_hi ^ x) << 4));
-            const uint32_t w[8] = {a.x, a.y, a.z, a.w, bq.x, bq.y, bq.z, bq.w};
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              v[2 * j] += p.s1 * bf16_lo(w[j]);
-              v[2 * j + 1] += p.s1 * bf16_hi(w[j]);
-            }
-          }
-          if (p.res2 != nullptr && valid) {
-            // second residual (only the temporal AlphaBlender GEMMs): read straight from global, own row
-            const __nv_bfloat16* rp = p.res2 + row * p.ld2 + ocol;
-            if (full) {
-              const uint4 a = __ldg(reinterpret_cast<const uint4*>(rp));
-              const uint4 bq = __ldg(reinterpret_cast<const uint4*>(rp) + 1);
-              const uint32_t w[8] = {a.x, a.y, a.z, a.w, bq.x, bq.y, bq.z, bq.w};
-#pragma unroll
-              for (int j = 0; j < 8; ++j) {
-                v[2 * j] += p.s2 * bf16_lo(w[j]);
-                v[2 * j + 1] += p.s2 * bf16_hi(w[j]);
-              }
-            } else {
-              for (int j = 0; j < 16; ++j)
-                if (ocol + j < n_out) v[j] += p.s2 * __bfloat162float(rp[j]);
-            }
-          }
-          *reinterpret_cast<uint4*>(orow + ((c_lo ^ x) << 4)) =
-              make_uint4(pack_bf16x2(v[0], v[1]), pack_bf16x2(v[2], v[3]), pack_bf16x2(v[4], v[5]), pack_bf16x2(v[6], v[7]));
-          *reinterpret_cast<uint4*>(orow + ((c_hi ^ x) << 4)) =
-              make_uint4(pack_bf16x2(v[8], v[9]), pack_bf16x2(v[10], v[11]), pack_bf16x2(v[12], v[13]),
-                         pack_bf16x2(v[14], v[15]));
-        }
-        fence_proxy_async_smem();  // generic-proxy smem writes -> visible to the TMA store
-      } else if (!skip) {
-        // direct epilogue: fp32 outputs (tiny GEMMs: embeddings, conv_out, attention scores)
-        for (uint32_t c0 = 0; c0 < subw; c0 += 16) {
-          const uint32_t acol = 64 * s + c0;
-          if (otile0 + acol >= n_out) break;
-          uint32_t va[16], vg[16];
-          tmem_ld16(tlane + acol, va);
-          if (geglu) tmem_ld16(tlane + (uint32_t)(BN / 2) + acol, vg);
-          tmem_ld_wait();
-          if (!valid) continue;
-          float v[16];
-#pragma unroll
-          for (int j = 0; j < 16; ++j) v[j] = __uint_as_float(va[j]);
-          const uint32_t ocol = otile0 + acol;
-          const bool full = (ocol + 16 <= n_out);
-          finish16(v, vg, n0 + acol, ocol, full);
-          if (p.res1 != nullptr) {
-            const __nv_bfloat16* rp = p.res1 + row * p.ld1 + ocol;
-            for (int j = 0; j < 16; ++j)
-              if (full || ocol + j < n_out) v[j] += p.s1 * __bfloat162float(rp[j]);
-          }
-          if (p.res2 != nullptr) {
-            const __nv_bfloat16* rp = p.res2 + row * p.ld2 + ocol;
-            for (int j = 0; j < 16; ++j)
-              if (full || ocol + j < n_out) v[j] += p.s2 * __bfloat162float(rp[j]);
-          }
-          if (p.out_fp32) {
-            float* op = reinterpret_cast<float*>(p.out) + row * p.ldo + ocol;
-            for (int j = 0; j < 16; ++j)
-              if (full || ocol + j < n_out) op[j] = v[j];
+          __nv_bfloat16* op = reinterpret_cast<__nv_bfloat16*>(p.out) + row[h] * p.ldo + ocol;
+          const uint32_t w = pack_bf16x2(v0, v1);
+          if (in1) {
+            *reinterpret_cast<uint32_t*>(op) = w;  // ldo % 8 == 0 and an even column: 4-byte aligned
           } else {
-            __nv_bfloat16* op = reinterpret_cast<__nv_bfloat16*>(p.out) + row * p.ldo + ocol;
-            for (int j = 0; j < 16; ++j)
-              if (full || ocol + j < n_out) op[j] = __float2bfloat16(v[j]);
+            op[0] = __float2bfloat16(v0);
           }
+          // statistics of the bf16-ROUNDED values, the ones the consumer reads
+          const float r0 = bf16_lo(w), r1 = in1 ? bf16_hi(w) : 0.f;
+          gs0 += r0;
+          gs1 += r1;
+          gq0 += r0 * r0;
+          gq1 += r1 * r1;
         }
       }
-      // this block's TMEM reads are done; the accumulator is handed back when the warp LEAVES the tile (with more than
-      // four 64-column sub-blocks per tile — the 320-wide tile — a warp owns two blocks of the same tile, and a second
-      // arrival for one tile would complete the barrier phase early)
-      tc_fence_before();
-      __syncwarp();
-      const uint32_t s_cur = s;
-      const uint32_t tprev = tcount;
-      s += 4;
-      while (s >= nsub_out) {
-        s -= nsub_out;
-        ++tcount;
-      }
-      if (lane == 0) {
-        if (tcount != tprev) {
-          if (PAIR) mbar_arrive_leader(&acc_empty[b]);
-          else mbar_arrive(&acc_empty[b]);
+      if (gn) {
+        // column sums over the warp's 16 rows (lanes of equal cq), then over the quadrant's two warps via smem
+#pragma unroll
+        for (int o = 4; o < 32; o <<= 1) {
+          gs0 += __shfl_xor_sync(0xffffffffu, gs0, o);
+          gs1 += __shfl_xor_sync(0xffffffffu, gs1, o);
+          gq0 += __shfl_xor_sync(0xffffffffu, gq0, o);
+          gq1 += __shfl_xor_sync(0xffffffffu, gq1, o);
         }
-        if (!skip && p.tma_epi) {
-          tma_store_5d(subw == 64 ? &tmO64 : &tmO32, ob, (int)ocol0, (int)(mb1 + qo1), (int)(mb2 + qo2),
-                       (int)(mb3 + qo3), 0);
-          tma_store_commit();
+        if (gn_sender && rq == 0)
+          *reinterpret_cast<float4*>(gxq + 2 * tcol) = make_float4(gs0, gq0, gs1, gq1);
+        if (!gn_sender) {
+          acc[4 * j] = gs0;  // the accumulators of this column block are consumed: park the partials there
+          acc[4 * j + 1] = gq0;
+          acc[4 * j + 2] = gs1;
+          acc[4 * j + 3] = gq1;
         }
-      }
-      (void)s_cur;
-      tpass = (tcount != tprev) ? tprev + 1 : tprev;
-      if (tcount < num_tiles) {
-        if (tcount != tprev) decode_tile(p, tile_begin + tcount, PAIR ? 2u : 1u, rank, QUAD ? 2u : 1u, npair, n_tile, mb1, mb2, mb3);
-        prefetch_residual();
       }
     }
-    for (; tpass < num_tiles; ++tpass) {
-      mbar_wait_parked(&acc_full[acc_buf(tpass)], acc_par(tpass));
-      if (lane == 0) {
-        if (PAIR) mbar_arrive_leader(&acc_empty[acc_buf(tpass)]);
-        else mbar_arrive(&acc_empty[acc_buf(tpass)]);
+    if (gn) {
+      named_bar_sync(gn_bar, 64);  // the partner warp's partials are in shared memory
+      if (!gn_sender) {
+        const uint32_t slot = (tile / p.n_tiles) * 4u + (uint32_t)quad;
+        if (rq == 0) {
+          float2* dst = reinterpret_cast<float2*>(p.gn_part) + (int64_t)slot * p.gn_ld;
+#pragma unroll
+          for (int j = 0; j < NJ; ++j) {
+            const uint32_t tcol = 8 * j + 2 * cq;
+            const uint32_t ocol = otile0 + tcol;
+            if (ocol < n_out) {
+              const float4 o = *reinterpret_cast<const float4*>(gxq + 2 * tcol);
+              dst[ocol] = make_float2(acc[4 * j] + o.x, acc[4 * j + 1] + o.y);
+              if (ocol + 1 < n_out) dst[ocol + 1] = make_float2(acc[4 * j + 2] + o.z, acc[4 * j + 3] + o.w);
+            }
+          }
+        }
+        // lane 0 holds the first row of the quadrant: if it is out of range, so is every row of the quadrant
+        if (lane == 0 && n_tile == 0) p.gn_slot_sample[slot] = valid[0] ? (int32_t)((uint32_t)row[0] / p.gn_rows) : -1;
       }
+      named_bar_sync(gn_bar, 64);  // read before the next tile overwrites
     }
-    if (p.tma_epi && lane == 0) tma_store_wait_all();  // all bulk stores of this thread have landed
-  }
-
-  tc_fence_before();
-  if (PAIR) cluster_sync_all();  // the peer may still be reading its accumulators / smem stages
-  else __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    if (PAIR) tmem_dealloc_2sm(tmem_base, Cfg::TMEM_COLS);
-    else tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
   }
 }
 
@@ -752,153 +358,44 @@ static int ilog2_exact(uint32_t v) {
   return l;
 }
 
-// rank-5 view of a row-major [rows][ld] bf16 matrix addressed through the output-pixel space:
-// dims (cols, M1, M2, M3, 1), element (col, m1, m2, m3) at base + (m1*rs0 + m2*rs1 + m3*rs2)*ld + col
-static int encode_rows_view(CUtensorMap* tm, const void* base, int64_t ld, uint32_t cols, const uint32_t* m_ext,
-                            const int64_t* rs, const uint32_t* box_rows, uint32_t box_cols) {
-  uint64_t dims[5] = {cols, m_ext[0], m_ext[1], m_ext[2], 1};
-  uint64_t str[4];
-  for (int i = 0; i < 3; ++i) {
-    // a size-1 dim may carry any stride; keep it a positive multiple of 16 bytes
-    const int64_t s = (m_ext[i] > 1 ? rs[i] : 1) * ld * 2;
-    if (s <= 0) {
-      set_error("b200svd_gemm: output row strides must be positive");
-      return 1;
-    }
-    str[i] = (uint64_t)s;
-  }
-  str[3] = str[2] * (m_ext[2] ? m_ext[2] : 1);
-  uint32_t box[5] = {box_cols, box_rows[0], box_rows[1], box_rows[2], 1};
-  return box_cols == 64 ? encode_tmap_bf16(tm, base, 5, dims, str, box) : encode_tmap_bf16_sw64(tm, base, 5, dims, str, box);
-}
-
-template <int BN, int CL, int EPI = 0>
+template <int BN>
 static int launch(const b200svd_gemm_params* p, const CUtensorMap& tmA, const GemmDev& d, cudaStream_t st) {
-  using Cfg = TileCfg<BN, CL>;
-  constexpr bool PAIR = CL >= 2;
-  constexpr bool QUAD = CL == 4;
-  // weights [taps][n][k] -> TMA dims (k, n, taps); in PAIR mode each CTA loads half of the N tile
+  using Cfg = TileCfg<BN>;
+  // weights [taps][n][k] -> TMA dims (k, n, taps)
   CUtensorMap tmB;
   uint64_t bd[3] = {p->k, p->n, p->taps};
   uint64_t bs[2] = {(uint64_t)p->k * 2, (uint64_t)p->k * 2 * p->n};
-  uint32_t bb[3] = {64, (uint32_t)(Cfg::B_ROWS / Cfg::NMMA), 1};
+  uint32_t bb[3] = {64, (uint32_t)BN, 1};
   if (encode_tmap_bf16(&tmB, p->w_ptr, 3, bd, bs, bb)) return 1;
   GemmDev dd = d;
   dd.n_tiles = (p->n + BN - 1) / BN;
-  if (QUAD) dd.n_tiles = (dd.n_tiles + 1) / 2;  // N work items = pairs of N tiles
-  // QUAD: second activation map whose box is one 64-row half of the A tile (outermost non-unit row dim halved)
-  CUtensorMap tmAh = tmA;
-  dd.a_half_dim = 0;
-  dd.a_half_size = 0;
-  if (QUAD) {
-    int hd = 2;
-    while (hd > 0 && p->m_box[hd] < 2) --hd;
-    if (p->m_box[hd] < 2) {
-      set_error("mtgemm: cannot halve the A tile");
-      return 1;
-    }
-    uint32_t hb[5];
-    for (int i = 0; i < 5; ++i) hb[i] = p->a_box[i];
-    dd.a_half_dim = p->m_adim[hd];
-    dd.a_half_size = p->m_box[hd] / 2;
-    hb[dd.a_half_dim] = dd.a_half_size;
-    if (encode_tmap_bf16(&tmAh, p->a_ptr, 5, p->a_dims, p->a_strides, hb)) return 1;
-  }
-
-  // epilogue tensor maps: output and residual-1, both in quadrant boxes of 32 rows
-  CUtensorMap tmO64, tmO32, tmR64, tmR32;
-  memset(&tmO64, 0, sizeof(tmO64));
-  tmO32 = tmO64;
-  tmR64 = tmO64;
-  tmR32 = tmO64;
-  if (dd.tma_epi) {
-    const uint32_t n_out = p->act == B200SVD_ACT_GEGLU ? p->n / 2 : p->n;
-    const uint32_t b1 = p->m_box[0], b2 = p->m_box[1];
-    const uint32_t c1 = b1 < 32 ? b1 : 32;
-    const uint32_t c2 = (b2 < 32 / c1) ? b2 : 32 / c1;
-    const uint32_t c3 = 32 / (c1 * c2);
-    const uint32_t qbox[3] = {c1, c2, c3};
-    if (encode_rows_view(&tmO64, p->out, p->ldo, n_out, p->m_ext, p->out_rs, qbox, 64)) return 1;
-    if (encode_rows_view(&tmO32, p->out, p->ldo, n_out, p->m_ext, p->out_rs, qbox, 32)) return 1;
-    if (p->res1 != nullptr) {
-      if (encode_rows_view(&tmR64, p->res1, p->ld1, n_out, p->m_ext, p->out_rs, qbox, 64)) return 1;
-      if (encode_rows_view(&tmR32, p->res1, p->ld1, n_out, p->m_ext, p->out_rs, qbox, 32)) return 1;
-    }
-  }
   const int slot = dev_slot();
   static bool attr_set[B200_MAX_DEVICES] = {};
   if (!attr_set[slot]) {
-    cudaError_t e = cudaFuncSetAttribute(mtgemm_kernel<BN, CL, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
+    cudaError_t e = cudaFuncSetAttribute(mtgemm_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
     if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(mtgemm)");
     attr_set[slot] = true;
   }
   const uint64_t m_tiles = (uint64_t)dd.m_tiles[0] * dd.m_tiles[1] * dd.m_tiles[2];
-  const uint64_t total = (uint64_t)dd.n_tiles * (PAIR ? (m_tiles + 1) / 2 : m_tiles);  // (pair) tiles
+  const uint64_t total = (uint64_t)dd.n_tiles * m_tiles;
   if (total == 0 || total > 0x7FFFFFFFull) {
     set_error("mtgemm: bad tile count %llu", (unsigned long long)total);
     return 1;
   }
-  // CTAs, CTA pairs or CTA quads that can be co-resident (clusters must fit inside a GPC, so quads may not tile all SMs)
-  static int max_clusters_dev[B200_MAX_DEVICES] = {};
-  int& max_clusters = max_clusters_dev[slot];
-  if (max_clusters == 0) {
-    max_clusters = sm_count() / CL;
-    if (CL > 1) {
-      cudaLaunchConfig_t qc = {};
-      qc.gridDim = dim3((unsigned)(sm_count() / CL * CL));
-      qc.blockDim = dim3(NUM_THREADS);
-      qc.dynamicSmemBytes = Cfg::SMEM_BYTES;
-      cudaLaunchAttribute qa[1];
-      qa[0].id = cudaLaunchAttributeClusterDimension;
-      qa[0].val.clusterDim.x = CL;
-      qa[0].val.clusterDim.y = 1;
-      qa[0].val.clusterDim.z = 1;
-      qc.attrs = qa;
-      qc.numAttrs = 1;
-      int nc = 0;
-      if (cudaOccupancyMaxActiveClusters(&nc, mtgemm_kernel<BN, CL, EPI>, &qc) == cudaSuccess && nc > 0 && nc < max_clusters)
-        max_clusters = nc;
-      else
-        (void)cudaGetLastError();
-    }
-  }
-  const uint32_t workers = (uint32_t)max_clusters;
-  const uint32_t nw = (uint32_t)(total < workers ? total : workers);
   dd.total_tiles = (uint32_t)total;
-  dd.tiles_per_cta = (uint32_t)((total + nw - 1) / nw);
-  const uint32_t used = (uint32_t)((total + dd.tiles_per_cta - 1) / dd.tiles_per_cta);
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(CL * used);
-  cfg.blockDim = dim3(NUM_THREADS);
-  cfg.dynamicSmemBytes = Cfg::SMEM_BYTES;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = CL;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  cudaError_t e = cudaLaunchKernelEx(&cfg, mtgemm_kernel<BN, CL, EPI>, tmA, tmAh, tmB, tmO64, tmO32, tmR64, tmR32, dd);
-  if (e != cudaSuccess) return cuda_fail(e, "mtgemm launch");
+  const uint32_t grid = (uint32_t)(total < (uint64_t)sm_count() ? total : (uint64_t)sm_count());
+  mtgemm_kernel<BN><<<grid, NUM_THREADS, Cfg::SMEM_BYTES, st>>>(tmA, tmB, dd);
+  B200_CHECK_LAUNCH("mtgemm launch");
   return 0;
 }
 
-// 0 = never, 1 = always (when the tile shape allows), 2 = auto (compute-heavy launches); env B200SVD_PAIR
-static int g_pair_mode = -1;
-static int pair_mode() {
-  if (g_pair_mode < 0) {
-    const char* e = getenv("B200SVD_PAIR");
-    g_pair_mode = e ? atoi(e) : 2;
-    if (g_pair_mode < 0 || g_pair_mode > 3) g_pair_mode = 2;
-  }
-  return g_pair_mode;
-}
+// Kept for the C ABI: CTA-pair (cta_group::2) tiles do not exist on sm_90, every launch uses single-CTA tiles.
+static int g_pair_mode = 2;
 
 }  // namespace b200
 
 extern "C" int b200svd_gemm_pair_mode(int mode) {
-  const int prev = b200::pair_mode();
+  const int prev = b200::g_pair_mode;
   if (mode >= 0 && mode <= 3) b200::g_pair_mode = mode;
   return prev;
 }
@@ -988,103 +485,42 @@ extern "C" int b200svd_gemm(const b200svd_gemm_params* p, void* stream) {
       return 1;
     }
   }
+  const uint64_t m_tiles_all = (uint64_t)d.m_tiles[0] * d.m_tiles[1] * d.m_tiles[2];
   if (bn == 0) {
     if (p->n <= 32) bn = 32;
     else if (p->n <= 64) bn = 64;
     else if (p->n <= 128) bn = 128;
-    // the pair tiles are bound by L2->SM bytes per FLOP (tools/bench_bn.py): the 256-wide tile wins even with a
-    // ragged last tile (its out-of-range weight rows are TMA zero fill, not traffic); N = 160 / 320 fit the 160 tile
-    else if (p->n == 160 || p->n == 320) bn = 160;
-    else bn = 256;
+    else if (p->n == 160 || p->n == 320) bn = 160;  // no ragged N tile
+    // a single M tile: the 128-wide tile spreads such a (weight-streaming) GEMM over more SMs
+    else bn = m_tiles_all < 2 ? 128 : 256;
   }
+  // wgmma takes N <= 256: a 320-wide tile is computed as two 160-wide tiles
+  if (bn == 320) bn = 160;
   auto al16 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
-  d.tma_epi = (!p->out_fp32 && p->ldo % 8 == 0 && al16(p->out) &&
-               (p->res1 == nullptr || (p->ld1 % 8 == 0 && al16(p->res1))) &&
-               (p->res2 == nullptr || (p->ld2 % 8 == 0 && al16(p->res2))))
-                  ? 1
-                  : 0;
-  if (!d.tma_epi && !p->out_fp32) {
+  const bool bf16_ok = p->ldo % 8 == 0 && al16(p->out) && (p->res1 == nullptr || (p->ld1 % 8 == 0 && al16(p->res1))) &&
+                       (p->res2 == nullptr || (p->ld2 % 8 == 0 && al16(p->res2)));
+  if (!p->out_fp32 && !bf16_ok) {
     set_error("b200svd_gemm: bf16 outputs/residuals need 16-byte aligned bases and leading dims that are multiples of 8");
+    return 1;
+  }
+  const uint32_t n_out = p->act == B200SVD_ACT_GEGLU ? p->n / 2 : p->n;
+  if (p->gn_part != nullptr &&
+      (p->act != B200SVD_ACT_NONE || p->out_fp32 || (n_out % 16) != 0 || bn < 128 || p->gn_slot_sample == nullptr ||
+       p->gn_ld < (int64_t)p->n || (p->gn_ld % 2) != 0 || (reinterpret_cast<uintptr_t>(p->gn_part) & 7) != 0)) {
+    set_error("b200svd_gemm: gn_part needs the activation-free bf16 epilogue (n %% 16 == 0, n > 64), gn_slot_sample and "
+              "an 8-byte aligned partial buffer with gn_ld >= n");
     return 1;
   }
 
   CUtensorMap tmA;
   if (encode_tmap_bf16(&tmA, p->a_ptr, 5, p->a_dims, p->a_strides, p->a_box)) return 1;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  // 2-SM (cta_group::2) tiles whenever a wide tile has at least two M tiles: measured neutral-to-better on every
-  // shape of the denoiser (profiles/r01_pair_shapes.txt); mode 1 additionally pairs the 128-wide tile
-  const uint64_t m_tiles_all = (uint64_t)d.m_tiles[0] * d.m_tiles[1] * d.m_tiles[2];
-  // a single M tile cannot pair: the 128-wide tile spreads such a (weight-streaming) GEMM over more SMs
-  if (p->bn == 0 && bn == 256 && m_tiles_all < 2 && p->act != B200SVD_ACT_GEGLU) bn = 128;
-  const int pm = pair_mode();
-  const bool pair = m_tiles_all >= 2 && ((pm >= 1 && (bn == 256 || bn == 160)) || (pm == 1 && bn == 128));
-  // mode 3: two pairs on adjacent N tiles share (multicast) their A tile when the N tile count is even
-  const uint32_t n_tiles_all = (p->n + (uint32_t)bn - 1) / (uint32_t)bn;
-  const bool quad = pair && pm == 3 && (n_tiles_all % 2) == 0;
-  // 320-wide pair tile (B200SVD_BN320=1; single-buffered accumulator): long main loops only
-  static int bn320 = -1;
-  if (bn320 < 0) {
-    const char* e = getenv("B200SVD_BN320");
-    bn320 = e ? atoi(e) : 0;
-  }
-  // measured (profiles/r02_bench_vs_libs*.txt): wins for N = 320 (convs 0.69 -> 0.57 ms, 1.96 -> 1.58 ms; FF2 0.39 -> 0.355)
-  // and for the N = 640 linears (0.353 -> 0.317); loses on the N = 640 / 1280 convolutions, whose 256-wide tiles are
-  // double-buffered
-  // mode 2 additionally takes the N = 640 convolutions (the 256-wide tile computes 768 columns for them: 17 % of the
-  // tensor work is spent on zero-filled weight rows)
-  if (bn320 && p->bn == 0 && (bn == 160 || bn == 256) &&
-      (p->n == 320 || (p->n == 640 && (p->taps == 1 || bn320 >= 2))) && m_tiles_all >= 2 && pm >= 1 &&
-      p->act == B200SVD_ACT_NONE && (uint64_t)p->taps * d.kblocks >= 15)
-    bn = 320;
-  // lean epilogue for everything without an activation (B200SVD_LEAN_EPI=0 keeps the generic loop: A/B knob)
-  static int lean_epi = -1;
-  if (lean_epi < 0) {
-    const char* e = getenv("B200SVD_LEAN_EPI");
-    lean_epi = e ? (atoi(e) != 0) : B200SVD_DEFAULT_LEAN_EPI;
-  }
-  const uint32_t n_out_h = p->act == B200SVD_ACT_GEGLU ? p->n / 2 : p->n;
-  const bool lean = lean_epi && p->act == B200SVD_ACT_NONE && d.tma_epi && (n_out_h % 16) == 0 &&
-                    (p->bias == nullptr || al16(p->bias)) &&
-                    (p->fvec == nullptr || (al16(p->fvec) && (p->ldf % 4) == 0)) && !quad;
-  if (p->gn_part != nullptr && (!lean || bn < 128 || p->gn_slot_sample == nullptr || p->gn_ld < (int64_t)p->n ||
-                                 (p->gn_ld % 2) != 0 || (reinterpret_cast<uintptr_t>(p->gn_part) & 7) != 0)) {
-    set_error("b200svd_gemm: gn_part needs the activation-free bf16 epilogue (n %% 16 == 0, n > 64), gn_slot_sample and "
-              "an 8-byte aligned partial buffer with gn_ld >= n");
-    return 1;
-  }
-  if (bn == 320) {
-    if (m_tiles_all < 2 || p->n % 320 != 0 || p->act == B200SVD_ACT_GEGLU) {
-      set_error("b200svd_gemm: the 320-wide tile is a 2-SM tile: needs >= 2 M tiles, n %% 320 == 0, no GEGLU");
-      return 1;
-    }
-    return lean ? launch<320, 2, 2>(p, tmA, d, st) : launch<320, 2, 0>(p, tmA, d, st);
-  }
-  if (lean) {
-    switch (bn) {
-      case 128: return pair ? launch<128, 2, 2>(p, tmA, d, st) : launch<128, 1, 2>(p, tmA, d, st);
-      case 160: return pair ? launch<160, 2, 2>(p, tmA, d, st) : launch<160, 1, 2>(p, tmA, d, st);
-      case 256: return pair ? launch<256, 2, 2>(p, tmA, d, st) : launch<256, 1, 2>(p, tmA, d, st);
-      default: break;
-    }
-  }
   switch (bn) {
-    case 32: return launch<32, 1>(p, tmA, d, st);
-    case 64: return launch<64, 1>(p, tmA, d, st);
-    case 128: return pair ? launch<128, 2>(p, tmA, d, st) : launch<128, 1>(p, tmA, d, st);
-    case 160:
-      return quad ? launch<160, 4>(p, tmA, d, st) : pair ? launch<160, 2>(p, tmA, d, st) : launch<160, 1>(p, tmA, d, st);
-    case 256: {
-      // specialised GEGLU epilogue (bias only); B200SVD_GEGLU_EPI=0 keeps the generic loop (A/B knob)
-      static int geglu_fast = -1;
-      if (geglu_fast < 0) {
-        const char* e = getenv("B200SVD_GEGLU_EPI");
-        geglu_fast = e ? (atoi(e) != 0) : B200SVD_DEFAULT_GEGLU_EPI;
-      }
-      const bool g1 = geglu_fast && p->act == B200SVD_ACT_GEGLU && d.tma_epi && p->bias != nullptr && al16(p->bias) &&
-                      p->fvec == nullptr && p->res1 == nullptr && p->res2 == nullptr && p->s_acc == 1.0f && !quad;
-      if (g1) return pair ? launch<256, 2, 1>(p, tmA, d, st) : launch<256, 1, 1>(p, tmA, d, st);
-      return quad ? launch<256, 4>(p, tmA, d, st) : pair ? launch<256, 2>(p, tmA, d, st) : launch<256, 1>(p, tmA, d, st);
-    }
+    case 32: return launch<32>(p, tmA, d, st);
+    case 64: return launch<64>(p, tmA, d, st);
+    case 128: return launch<128>(p, tmA, d, st);
+    case 160: return launch<160>(p, tmA, d, st);
+    case 256: return launch<256>(p, tmA, d, st);
     default: set_error("b200svd_gemm: unsupported N tile %d", bn); return 1;
   }
 }

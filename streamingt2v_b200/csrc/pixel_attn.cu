@@ -4,12 +4,11 @@
 // Replaces VideoTransformerBlock.attn1 (reference code/models/svd/sgm/modules/video_attention.py:145-148, after the
 // "(b t) s c -> (b s) t c" transpose of :131) and the CAM CrossAttention core (code/models/cam/conditioning.py:65-68).
 //
-// One CTA = 4 pixels x 1 head.  The 4 x 32 (frames padded to 32) query rows form one 128-row tile, the 4 x 32 key rows
-// one 128-key block; S = Q K^T is computed for the whole tile by tcgen05.mma and only the block diagonal (same pixel)
-// is kept.  The frame-strided rows of a pixel are gathered by TMA (box = 64 channels x 1 pixel x 32 frames; frames
-// beyond L are zero-filled), so the reference's transpose never exists in HBM.  TMEM use is 128 columns: S in
-// [0,128); P (packed bf16) overwrites [0,64) and O accumulates in [64,128) once S has been read, so four CTAs
-// co-reside per SM and hide each other's TMA / MMA latency.
+// One CTA = 4 pixels x 1 head, two warpgroups of two pixels each.  The 2 x 32 (frames padded to 32) query rows of a
+// warpgroup form one 64-row wgmma tile, the same pixels' 2 x 32 key rows one 64-key block; S = Q K^T is computed for
+// the whole block by wgmma and only the block diagonal (same pixel) is kept.  The frame-strided rows of a pixel are
+// gathered by TMA (box = 64 channels x 1 pixel x 32 frames; frames beyond L are zero-filled), so the reference's
+// transpose never exists in HBM.  Softmax and P stay in registers; P is the register A operand of O = P V.
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <math.h>
@@ -17,13 +16,13 @@
 #include "../../include/b200svd.h"
 #include "common.h"
 #include "ptx.cuh"
+#include "wgmma.cuh"
 
 namespace b200 {
 
-constexpr int PA_TILE_BYTES = 128 * 64 * 2;  // 16 KB: Q, K, V tiles
+constexpr int PA_TILE_BYTES = 128 * 64 * 2;  // 16 KB: Q, K, V tiles of 4 pixels
 constexpr int PA_SMEM_BYTES = 3 * PA_TILE_BYTES + 128;
-constexpr int PA_TMEM_COLS = 128;
-constexpr int PA_THREADS = 6 * 32;
+constexpr int PA_THREADS = 2 * 128;
 
 struct PaParams {
   __nv_bfloat16* out;
@@ -32,7 +31,7 @@ struct PaParams {
   float scale_log2;
 };
 
-__global__ void __launch_bounds__(PA_THREADS, 4)
+__global__ void __launch_bounds__(PA_THREADS)
 pixel_attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                   const __grid_constant__ CUtensorMap tmV, const PaParams p) {
   extern __shared__ __align__(1024) uint8_t smem[];
@@ -40,140 +39,109 @@ pixel_attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant
   uint8_t* sQ = smem;
   uint8_t* sK = sQ + PA_TILE_BYTES;
   uint8_t* sV = sK + PA_TILE_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sV + PA_TILE_BYTES);
-  uint64_t* ld_full = bars;
-  uint64_t* s_full = bars + 1;
-  uint64_t* p_full = bars + 2;
-  uint64_t* o_full = bars + 3;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 4);
+  uint64_t* ld_full = reinterpret_cast<uint64_t*>(sV + PA_TILE_BYTES);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int pix0 = blockIdx.x * 4, head = blockIdx.y, b = blockIdx.z;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     prefetch_tmap(&tmQ);
     prefetch_tmap(&tmK);
     prefetch_tmap(&tmV);
     mbar_init(ld_full, 1);
-    mbar_init(s_full, 1);
-    mbar_init(p_full, 4);
-    mbar_init(o_full, 1);
     fence_barrier_init();
   }
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, PA_TMEM_COLS);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
+  if (threadIdx.x == 0) {
+    // TMA: 4 pixels x {Q, K, V}; each box = 64 channels x 1 pixel x 32 frames -> 4 KB, rows ordered (pixel, frame)
+    mbar_expect_tx(ld_full, 3 * PA_TILE_BYTES);
+#pragma unroll
+    for (int px = 0; px < 4; ++px) {
+      tma_load_4d(sQ + px * 4096, &tmQ, ld_full, head * 64, pix0 + px, 0, b);
+      tma_load_4d(sK + px * 4096, &tmK, ld_full, head * 64, pix0 + px, 0, b);
+      tma_load_4d(sV + px * 4096, &tmV, ld_full, head * 64, pix0 + px, 0, b);
+    }
+  }
+  // warpgroup cw: pixels 2 cw, 2 cw + 1 of the CTA; warp wl: 16 query rows of pixel wl / 2
+  const int cw = warp >> 2, wl = warp & 3;
+  const int rq = lane >> 2, cq = lane & 3;
+  const int wpix = wl >> 1;  // pixel of this warp's rows inside the warpgroup
+  mbar_wait(ld_full, 0);
 
-  if (warp == 0) {
-    if (lane == 0) {
-      // TMA: 4 pixels x {Q, K, V}; each box = 64 channels x 1 pixel x 32 frames -> 4 KB, rows ordered (pixel, frame)
-      mbar_expect_tx(ld_full, 3 * PA_TILE_BYTES);
+  float sacc[32];
 #pragma unroll
-      for (int px = 0; px < 4; ++px) {
-        tma_load_4d(sQ + px * 4096, &tmQ, ld_full, head * 64, pix0 + px, 0, b);
-        tma_load_4d(sK + px * 4096, &tmK, ld_full, head * 64, pix0 + px, 0, b);
-        tma_load_4d(sV + px * 4096, &tmV, ld_full, head * 64, pix0 + px, 0, b);
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc_qk = make_idesc_f16(128, 128, 1, 0, 0);
-      constexpr uint32_t idesc_pv = make_idesc_f16(128, 64, 1, 0, 1);  // B (=V) is MN-major
-      mbar_wait(ld_full, 0);
-      tc_fence_after();
-      const uint64_t qdesc = smem_desc_k_sw128(smem_u32(sQ));
-      const uint64_t kdesc = smem_desc_k_sw128(smem_u32(sK));
+  for (int i = 0; i < 32; ++i) sacc[i] = 0.f;
+  const uint64_t qdesc = smem_desc_k_sw128(smem_u32(sQ + cw * 8192));
+  const uint64_t kdesc = smem_desc_k_sw128(smem_u32(sK + cw * 8192));
+  wgmma_fence_regs(sacc);
+  wgmma_fence();
 #pragma unroll
-      for (int kk = 0; kk < 4; ++kk) umma_f16_ss(tmem_base, qdesc + kk * 2, kdesc + kk * 2, idesc_qk, kk > 0);
-      umma_commit(s_full);
-      mbar_wait(p_full, 0);
-      tc_fence_after();
-      const uint64_t vdesc = smem_desc_mn_sw128(smem_u32(sV));
-#pragma unroll
-      for (int kk = 0; kk < 8; ++kk)
-        umma_f16_ts(tmem_base + 64, tmem_base + kk * 8, vdesc + (uint64_t)(kk * 128), idesc_pv, kk > 0);
-      umma_commit(o_full);
-    }
-    __syncwarp();
-  } else {
-    // softmax warps 2..5: TMEM lane quadrant qd == pixel index inside the tile; lane == frame
-    const int qd = warp & 3;
-    const uint32_t tl = ((uint32_t)(qd * 32)) << 16;
-    mbar_wait(s_full, 0);
-    tc_fence_after();
-    uint32_t sv[32];
-    tmem_ld32(tmem_base + tl + qd * 32, sv);  // only the block-diagonal 32 columns of this pixel
-    tmem_ld_wait();
-    float mx = -INFINITY;
-#pragma unroll
-    for (int i = 0; i < 32; ++i)
-      if (i < p.Lk) mx = fmaxf(mx, __uint_as_float(sv[i]));
-    const float mb = mx * p.scale_log2;
+  for (int kk = 0; kk < 4; ++kk) Wgmma<64>::ss(sacc, qdesc + (uint64_t)(kk * 2), kdesc + (uint64_t)(kk * 2), 1u);
+  wgmma_commit();
+  wgmma_wait<0>();
+  wgmma_fence_regs(sacc);
+
+  // keep the block diagonal: key column 8 jj + 2 cq + e belongs to pixel jj / 4, frame (8 jj + 2 cq + e) % 32
+  uint32_t pa[4][4];
+  float inv[2];
+  {
     float pr[32];
-    float l = 0.f;
 #pragma unroll
-    for (int i = 0; i < 32; ++i) {
-      pr[i] = (i < p.Lk) ? ex2_approx(fmaf(__uint_as_float(sv[i]), p.scale_log2, -mb)) : 0.f;
-      l += pr[i];
+    for (int h = 0; h < 2; ++h) {
+      float mx = -INFINITY;
+#pragma unroll
+      for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+        for (int e = 0; e < 2; ++e)
+          if ((jj >> 2) == wpix && ((8 * jj + 2 * cq + e) & 31) < p.Lk) mx = fmaxf(mx, sacc[4 * jj + 2 * h + e]);
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+      const float mb = mx * p.scale_log2;
+      float l = 0.f;
+#pragma unroll
+      for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const bool keep = (jj >> 2) == wpix && ((8 * jj + 2 * cq + e) & 31) < p.Lk;
+          const float v = keep ? ex2_approx(fmaf(sacc[4 * jj + 2 * h + e], p.scale_log2, -mb)) : 0.f;
+          pr[4 * jj + 2 * h + e] = v;
+          l += v;
+        }
+      l += __shfl_xor_sync(0xffffffffu, l, 1);
+      l += __shfl_xor_sync(0xffffffffu, l, 2);
+      inv[h] = 1.0f / l;
     }
-    const float inv = 1.0f / l;
-    // P row: 128 keys packed as 64 words; only words [16*qd, 16*qd+16) are non-zero (normalised probabilities)
-    uint32_t w0[32], w1[32];
+    // normalised probabilities as the A operand of m64k16 (accumulator layout of two 8-column blocks)
 #pragma unroll
-    for (int i = 0; i < 32; ++i) {
-      w0[i] = 0u;
-      w1[i] = 0u;
-    }
-#pragma unroll
-    for (int i = 0; i < 16; ++i) {
-      const uint32_t v = pack_bf16x2(pr[2 * i] * inv, pr[2 * i + 1] * inv);
-      if (qd == 0) w0[i] = v;
-      else if (qd == 1) w0[16 + i] = v;
-      else if (qd == 2) w1[i] = v;
-      else w1[16 + i] = v;
-    }
-    tmem_st32(tmem_base + tl + 0, w0);
-    tmem_st32(tmem_base + tl + 32, w1);
-    tmem_st_wait();
-    tc_fence_before();
-    __syncwarp();
-    if (lane == 0) mbar_arrive(p_full);
-
-    mbar_wait(o_full, 0);
-    tc_fence_after();
-    uint32_t oa[32], ob[32];
-    tmem_ld32(tmem_base + tl + 64, oa);
-    tmem_ld32(tmem_base + tl + 96, ob);
-    tmem_ld_wait();
-    const int pix = pix0 + qd;
-    if (lane < p.Lq && pix < p.S) {
-      __nv_bfloat16* dst = p.out + (((int64_t)b * p.Lq + lane) * p.S + pix) * p.ldo + head * 64;
-#pragma unroll
-      for (int cc = 0; cc < 4; ++cc) {
-        reinterpret_cast<uint4*>(dst)[cc] = make_uint4(
-            pack_bf16x2(__uint_as_float(oa[8 * cc]), __uint_as_float(oa[8 * cc + 1])),
-            pack_bf16x2(__uint_as_float(oa[8 * cc + 2]), __uint_as_float(oa[8 * cc + 3])),
-            pack_bf16x2(__uint_as_float(oa[8 * cc + 4]), __uint_as_float(oa[8 * cc + 5])),
-            pack_bf16x2(__uint_as_float(oa[8 * cc + 6]), __uint_as_float(oa[8 * cc + 7])));
-        reinterpret_cast<uint4*>(dst)[4 + cc] = make_uint4(
-            pack_bf16x2(__uint_as_float(ob[8 * cc]), __uint_as_float(ob[8 * cc + 1])),
-            pack_bf16x2(__uint_as_float(ob[8 * cc + 2]), __uint_as_float(ob[8 * cc + 3])),
-            pack_bf16x2(__uint_as_float(ob[8 * cc + 4]), __uint_as_float(ob[8 * cc + 5])),
-            pack_bf16x2(__uint_as_float(ob[8 * cc + 6]), __uint_as_float(ob[8 * cc + 7])));
-      }
+    for (int kk = 0; kk < 4; ++kk) {
+      pa[kk][0] = pack_bf16x2(pr[8 * kk + 0] * inv[0], pr[8 * kk + 1] * inv[0]);
+      pa[kk][1] = pack_bf16x2(pr[8 * kk + 2] * inv[1], pr[8 * kk + 3] * inv[1]);
+      pa[kk][2] = pack_bf16x2(pr[8 * kk + 4] * inv[0], pr[8 * kk + 5] * inv[0]);
+      pa[kk][3] = pack_bf16x2(pr[8 * kk + 6] * inv[1], pr[8 * kk + 7] * inv[1]);
     }
   }
+  float o[32];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) o[i] = 0.f;
+  const uint64_t vdesc = smem_desc_mn_sw128(smem_u32(sV + cw * 8192));
+  wgmma_fence_regs(o);
+  wgmma_fence();
+#pragma unroll
+  for (int kk = 0; kk < 4; ++kk) Wgmma<64>::rs_tb(o, pa[kk], vdesc + (uint64_t)(kk * 128), 1u);
+  wgmma_commit();
+  wgmma_wait<0>();
+  wgmma_fence_regs(o);
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, PA_TMEM_COLS);
+  const int pix = pix0 + 2 * cw + wpix;
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int frame = (16 * wl + rq + 8 * h) & 31;
+    if (frame < p.Lq && pix < p.S) {
+      __nv_bfloat16* dst = p.out + (((int64_t)b * p.Lq + frame) * p.S + pix) * p.ldo + head * 64 + 2 * cq;
+#pragma unroll
+      for (int jj = 0; jj < 8; ++jj)
+        *reinterpret_cast<uint32_t*>(dst + 8 * jj) = pack_bf16x2(o[4 * jj + 2 * h], o[4 * jj + 2 * h + 1]);
+    }
   }
 }
 

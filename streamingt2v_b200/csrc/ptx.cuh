@@ -1,4 +1,4 @@
-// Thin inline-PTX wrappers for sm_100a: mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (MMA / TMEM).
+// Thin inline-PTX wrappers for sm_90a: mbarrier, TMA (cp.async.bulk.tensor), wgmma descriptors.
 // Everything here is device-side and header-only.  No CUTLASS dependency.
 #pragma once
 #include <cuda.h>
@@ -21,7 +21,7 @@ __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
 __device__ __forceinline__ void fence_barrier_init() {
   asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
 }
-// make generic-proxy smem writes visible to the async proxy (TMA / tcgen05 operand reads)
+// make generic-proxy smem writes visible to the async proxy (TMA / wgmma operand reads)
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
@@ -124,191 +124,17 @@ __device__ __forceinline__ void named_bar_arrive(int id, int nthreads) {
 }
 
 // ----------------------------------------------------------------------------------------------
-// tcgen05: TMEM allocation, MMA, commit, TMEM loads
-// ----------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {  // whole warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {  // whole warp
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem desc] * B[smem desc], kind::f16 (bf16/fp16 inputs, fp32 accumulate). One thread issues.
-__device__ __forceinline__ void umma_f16_ss(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                            uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// A operand from TMEM (packed 16-bit), B from smem.
-__device__ __forceinline__ void umma_f16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc, uint32_t idesc,
-                                            uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "r"(tmem_a), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// mbarrier arrive when all previously issued tcgen05.mma of this thread have completed
-// (implies tcgen05.fence::before_thread_sync).
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-
-// TMEM -> registers: this warp's 32 lanes x 16 consecutive 32-bit columns (lane = row).
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, "
-      "%15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, "
-      "%15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-        "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-        "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-}
-// wait::ld that also names the destination registers: the loads complete asynchronously, so every use of the values
-// must be ordered after the wait — as operands they are, for the compiler too (software-pipelined loads).
-__device__ __forceinline__ void tmem_ld_wait32(uint32_t (&v)[32]) {
-  asm volatile("tcgen05.wait::ld.sync.aligned;"
-               : "+r"(v[0]), "+r"(v[1]), "+r"(v[2]), "+r"(v[3]), "+r"(v[4]), "+r"(v[5]), "+r"(v[6]), "+r"(v[7]),
-                 "+r"(v[8]), "+r"(v[9]), "+r"(v[10]), "+r"(v[11]), "+r"(v[12]), "+r"(v[13]), "+r"(v[14]), "+r"(v[15]),
-                 "+r"(v[16]), "+r"(v[17]), "+r"(v[18]), "+r"(v[19]), "+r"(v[20]), "+r"(v[21]), "+r"(v[22]), "+r"(v[23]),
-                 "+r"(v[24]), "+r"(v[25]), "+r"(v[26]), "+r"(v[27]), "+r"(v[28]), "+r"(v[29]), "+r"(v[30]), "+r"(v[31])
-               :
-               : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// registers -> TMEM (this warp's 32 lanes x 16 columns)
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, "
-      "%15, %16};" ::"r"(taddr),
-      "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]),
-      "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, "
-      "%15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};" ::"r"(taddr),
-      "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]),
-      "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15]), "r"(v[16]), "r"(v[17]), "r"(v[18]),
-      "r"(v[19]), "r"(v[20]), "r"(v[21]), "r"(v[22]), "r"(v[23]), "r"(v[24]), "r"(v[25]), "r"(v[26]), "r"(v[27]),
-      "r"(v[28]), "r"(v[29]), "r"(v[30]), "r"(v[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// ----------------------------------------------------------------------------------------------
-// 2-SM (CTA pair, cta_group::2) variants.  Shared-window addresses carry the CTA rank of the cluster in bit 24;
-// clearing it addresses the same offset in the even ("leader") CTA of the pair.
-// ----------------------------------------------------------------------------------------------
-constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_alloc_2sm(uint32_t* dst_smem, uint32_t ncols) {  // one warp in EACH CTA of the pair
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish_2sm() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_2sm(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// TMA loads whose completion bytes are credited to the LEADER CTA's mbarrier (same offset)
-__device__ __forceinline__ void tma_load_5d_2sm(void* smem, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2,
-                                                int c3, int c4) {
-  asm volatile(
-      "cp.async.bulk.tensor.5d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, "
-      "%5, %6, %7}], [%2];" ::"r"(smem_u32(smem)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_3d_2sm(void* smem, const CUtensorMap* m, uint64_t* bar, int c0, int c1,
-                                                int c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, "
-      "%5}], [%2];" ::"r"(smem_u32(smem)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1), "r"(c2)
-      : "memory");
-}
-// D[tmem, both CTAs] (+)= A[each CTA's smem: its 128 rows] * B[N split across the pair]; issued by the leader CTA only
-__device__ __forceinline__ void umma_f16_ss_2sm(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                                uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// commit -> arrive on the mbarrier at this offset in BOTH CTAs of the pair
-__device__ __forceinline__ void umma_commit_2sm(uint64_t* bar, uint16_t cta_mask = 3) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-                   smem_u32(bar)),
-               "h"(cta_mask)
-               : "memory");
-}
-// 2-SM tiled load multicast to the CTAs of cta_mask (same smem offset in each); every destination's bytes are
-// credited to the barrier of the leader of ITS pair
-__device__ __forceinline__ void tma_load_5d_2sm_mc(void* smem, const CUtensorMap* m, uint64_t* bar, int c0, int c1,
-                                                   int c2, int c3, int c4, uint16_t cta_mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.5d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], "
-      "[%1, {%4, %5, %6, %7, %8}], [%2], %3;" ::"r"(smem_u32(smem)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar) & kPeerBitMask), "h"(cta_mask), "r"(c0), "r"(c1), "r"(c2),
-      "r"(c3), "r"(c4)
-      : "memory");
-}
-// arrive on the leader CTA's mbarrier (from either CTA of the pair)
-__device__ __forceinline__ void mbar_arrive_leader(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(smem_u32(bar) & kPeerBitMask) : "memory");
-}
-
-// ----------------------------------------------------------------------------------------------
 // Descriptors
 // ----------------------------------------------------------------------------------------------
-// Shared-memory matrix descriptor, K-major operand, 128-byte swizzle, rows of 64 x 16-bit (=128 B), 8-row groups
-// 1024 B apart (dense tile written by a SWIZZLE_128B TMA box whose inner extent is 64 elements).
+// wgmma shared-memory matrix descriptor, K-major operand, 128-byte swizzle: rows of 64 x 16-bit (= 128 B), 8-row
+// groups 1024 B apart (the dense tile a SWIZZLE_128B TMA box with a 64-element inner extent writes).  Stepping 16
+// elements along K inside the swizzle atom adds 32 B (+2 in the address field).
 __device__ __forceinline__ uint64_t smem_desc_k_sw128(uint32_t saddr) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr >> 4) & 0x3FFF);  // start address  [0,14)
   d |= (uint64_t)1 << 16;                  // LBO (unused for swizzled K-major) = 1
   d |= (uint64_t)(1024 >> 4) << 32;        // SBO = 1024 B  [32,46)
-  d |= (uint64_t)1 << 46;                  // descriptor version (Blackwell)
-  d |= (uint64_t)2 << 61;                  // SWIZZLE_128B
+  d |= (uint64_t)1 << 62;                  // layout type SWIZZLE_128B  [62,64)
   return d;
 }
 // MN-major operand, 128-byte swizzle: smem tile is [K rows][64 MN elements = 128 B]; 8-row (K) groups 1024 B apart.
@@ -317,15 +143,8 @@ __device__ __forceinline__ uint64_t smem_desc_mn_sw128(uint32_t saddr) {
   d |= (uint64_t)((saddr >> 4) & 0x3FFF);
   d |= (uint64_t)1 << 16;            // LBO: stride between 64-element MN atoms (single atom here)
   d |= (uint64_t)(1024 >> 4) << 32;  // SBO: stride between 8-deep K groups
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
+  d |= (uint64_t)1 << 62;
   return d;
-}
-// Instruction descriptor, kind::f16, D = f32.  ab_fmt: 0 = f16, 1 = bf16.  b_mn_major: B operand MN-major.
-__host__ __device__ constexpr uint32_t make_idesc_f16(uint32_t M, uint32_t N, uint32_t ab_fmt, uint32_t a_mn_major,
-                                                     uint32_t b_mn_major) {
-  return (1u << 4) | (ab_fmt << 7) | (ab_fmt << 10) | (a_mn_major << 15) | (b_mn_major << 16) | ((N >> 3) << 17) |
-         ((M >> 4) << 24);
 }
 
 // ----------------------------------------------------------------------------------------------
@@ -339,68 +158,6 @@ __device__ __forceinline__ float ex2_approx(float x) {
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
-// 2^x on the FMA/ALU pipes (no MUFU): round-to-nearest split x = n + f, |f| <= 0.5, cubic for 2^f (rel err < 7e-4,
-// below the bf16 rounding the attention probabilities get anyway), exponent patched in with one integer add.
-// Valid for x <= 127; x below -126 is clamped (result ~1e-38).
-__device__ __forceinline__ float ex2_poly(float x) {
-  x = fmaxf(x, -126.0f);
-  const float t = x + 12582912.0f;  // 1.5 * 2^23: the low mantissa bits now hold round(x)
-  const float f = x - (t - 12582912.0f);
-  float pl = fmaf(0.0555041f, f, 0.2402265f);
-  pl = fmaf(pl, f, 0.6931472f);
-  pl = fmaf(pl, f, 1.0f);
-  return __uint_as_float(__float_as_uint(pl) + (__float_as_uint(t) << 23));
-}
-// ---- packed fp32 pairs (FFMA2 / FADD2: two fp32 lanes per instruction on sm_100) and 3-input max (FMNMX3) ----
-struct f32x2 {
-  uint64_t v;
-};
-__device__ __forceinline__ f32x2 pack2(float lo, float hi) {
-  f32x2 r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r.v) : "f"(lo), "f"(hi));
-  return r;
-}
-__device__ __forceinline__ f32x2 pack2u(uint32_t lo, uint32_t hi) {
-  f32x2 r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r.v) : "r"(lo), "r"(hi));
-  return r;
-}
-__device__ __forceinline__ void unpack2(f32x2 a, float& lo, float& hi) {
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(a.v));
-}
-__device__ __forceinline__ f32x2 fma2(f32x2 a, f32x2 b, f32x2 c) {
-  f32x2 r;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r.v) : "l"(a.v), "l"(b.v), "l"(c.v));
-  return r;
-}
-__device__ __forceinline__ f32x2 add2(f32x2 a, f32x2 b) {
-  f32x2 r;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r.v) : "l"(a.v), "l"(b.v));
-  return r;
-}
-__device__ __forceinline__ float max3f(float a, float b, float c) {
-  float d;
-  asm("max.f32 %0, %1, %2, %3;" : "=f"(d) : "f"(a), "f"(b), "f"(c));
-  return d;
-}
-// exp2 of a PAIR on the FMA pipe (same polynomial as ex2_poly): 5 packed FMA-pipe instructions + 2 clamps + 2 integer
-// exponent patches for two results, against 2 MUFU instructions.
-__device__ __forceinline__ void ex2_poly2(f32x2 x, float& ra, float& rb) {
-  float xa, xb;
-  unpack2(x, xa, xb);
-  x = pack2(fmaxf(xa, -126.0f), fmaxf(xb, -126.0f));
-  const f32x2 magic = pack2(12582912.0f, 12582912.0f), nmagic = pack2(-12582912.0f, -12582912.0f);
-  const f32x2 t = add2(x, magic);                       // low mantissa bits hold round(x)
-  const f32x2 f = fma2(add2(t, nmagic), pack2(-1.0f, -1.0f), x);   // x - round(x) in [-0.5, 0.5]
-  f32x2 pl = fma2(pack2(0.0555041f, 0.0555041f), f, pack2(0.2402265f, 0.2402265f));
-  pl = fma2(pl, f, pack2(0.6931472f, 0.6931472f));
-  pl = fma2(pl, f, pack2(1.0f, 1.0f));
-  float pa, pb, ta, tb;
-  unpack2(pl, pa, pb);
-  unpack2(t, ta, tb);
-  ra = __uint_as_float(__float_as_uint(pa) + (__float_as_uint(ta) << 23));
-  rb = __uint_as_float(__float_as_uint(pb) + (__float_as_uint(tb) << 23));
-}
 __device__ __forceinline__ float rcp_approx(float x) {
   float y;
   asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
@@ -411,7 +168,7 @@ __device__ __forceinline__ float gelu_f(float x) {  // exact (erf) GELU, matches
 }
 // GELU(x) = x * Phi(x) with erf via Abramowitz-Stegun 7.1.25 (|abs err| <= 2.5e-5, two orders below the bf16 output
 // rounding): 2 MUFU + 10 FMA-pipe instructions, branch free.  erff's ~35 instructions made the GEGLU epilogue
-// issue-bound (profiles/r01_ncu_v4_geglu_details.txt).
+// issue-bound.
 //   gelu = h + |h| * erf(|x|/sqrt2),  h = x/2;  erf(z) = 1 - (a1 t + a2 t^2 + a3 t^3) exp(-z^2),  t = 1/(1 + p z)
 __device__ __forceinline__ float gelu_fast(float x) {
   const float t = rcp_approx(fmaf(0.47047f * 0.70710678118654752440f, fabsf(x), 1.0f));
@@ -422,33 +179,6 @@ __device__ __forceinline__ float gelu_fast(float x) {
   const float h = 0.5f * x;
   const float pe = poly * e;
   return fmaf(-fabsf(h), pe, h + fabsf(h));
-}
-__device__ __forceinline__ f32x2 mul2(f32x2 a, f32x2 b) {
-  f32x2 r;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r.v) : "l"(a.v), "l"(b.v));
-  return r;
-}
-__device__ __forceinline__ f32x2 splat2(float a) { return pack2(a, a); }
-// value * GELU(gate) for a PAIR (GEGLU, attention.py:94-101), same A&S 7.1.25 erf as gelu_fast with the polynomial,
-// the scalings and the blend on packed FFMA2/FMUL2: 11 packed + 2 ALU + 4 MUFU instructions per pair (gelu_fast + the
-// product: 26 per pair).  gelu(g) = h + |h| erf(|g|/sqrt2), h = g/2; the polynomial is evaluated NEGATED so that
-// the last step is one fma: h + |h| + |h| * (-(poly * e)).
-__device__ __forceinline__ f32x2 geglu2(f32x2 v, f32x2 g) {
-  float g0, g1;
-  unpack2(g, g0, g1);
-  const f32x2 ax = pack2(fabsf(g0), fabsf(g1));
-  float d0, d1;
-  unpack2(fma2(ax, splat2(0.47047f * 0.70710678118654752440f), splat2(1.0f)), d0, d1);
-  const f32x2 t = pack2(rcp_approx(d0), rcp_approx(d1));
-  f32x2 np = fma2(splat2(-0.7478556f), t, splat2(0.0958798f));
-  np = fma2(np, t, splat2(-0.3480242f));
-  np = mul2(np, t);                                                   // -(a1 t + a2 t^2 + a3 t^3)
-  float z0, z1;
-  unpack2(mul2(mul2(g, g), splat2(-0.5f * 1.4426950408889634f)), z0, z1);
-  const f32x2 npe = mul2(np, pack2(ex2_approx(z0), ex2_approx(z1)));  // -poly * exp(-g^2/2)
-  const f32x2 ah = mul2(ax, splat2(0.5f));
-  const f32x2 hp = fma2(g, splat2(0.5f), ah);                         // h + |h|
-  return mul2(fma2(ah, npe, hp), v);
 }
 __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
   __nv_bfloat162 t = __floats2bfloat162_rn(lo, hi);

@@ -1,4 +1,4 @@
-"""Host-side executor of the StreamingSVD denoiser on the B200 kernels.
+"""Host-side executor of the StreamingSVD denoiser on the project's sm_90a kernels.
 
 Mirrors, op for op, the reference call tree under `StreamingWrapper.forward`
 (code/models/diffusion/wrappers.py:23-78 -> controlnet.py:496-554 + video_model.py:540-618) but
@@ -172,7 +172,7 @@ class _NetWeights:
 
 
 class B200Denoiser:
-    """ControlNet + VideoUNet(+CAM) forward on the B200 kernels.  See module docstring."""
+    """ControlNet + VideoUNet(+CAM) forward on the project's sm_90a kernels.  See module docstring."""
 
     def __init__(self, cfg: UNetConfig, sd_unet: SD, sd_ctrl: Optional[SD], device):
         ops._lib.init(torch.device(device).index or 0)

@@ -1,7 +1,7 @@
 """Op-level host wrappers over the C ABI (ctypes): build the TMA views / tap tables and launch.
 
 All activations are bf16, channel-last ("(b t) h w c" == token rows "(b t) (h w) c").  Nothing here computes on
-the host; every function enqueues one hand-written sm_100a kernel on torch's current CUDA stream.
+the host; every function enqueues one hand-written sm_90a kernel on torch's current CUDA stream.
 """
 from __future__ import annotations
 
@@ -25,13 +25,13 @@ def launches() -> int:
 
 
 def gemm_pair_mode(mode: int = -1) -> int:
-    """Set when the wide GEMM tiles run as 2-SM (cta_group::2) tiles: 0 never, 1 whenever possible, 2 automatic.
+    """Records a CTA-pair tile mode (0..3; kept for ABI compatibility: sm_90 runs single-CTA tiles in every mode).
     Any other value only queries.  Returns the previous mode."""
     return int(_lib.load().b200svd_gemm_pair_mode(int(mode)))
 
 
 def flash_attn_variant(v: int = -1) -> int:
-    """Softmax organisation of flash_attn: 3 two-pass, 4 single optimistic pass (default), 5 sixteen softmax warps.
+    """Records a softmax variant (3..5; kept for ABI compatibility: the sm_90 kernel has one softmax organisation).
     Any other value only queries.  Returns the previous variant."""
     return int(_lib.load().b200svd_flash_attn_variant(int(v)))
 
@@ -179,11 +179,9 @@ def gemm_raw(*, a, a_dims, a_strides, a_box, w, n, k, taps, tap_off, m_ext, m_bo
         _prof_end(e0, ("mtgemm", desc), 2.0 * rows * k * n * taps, nbytes)
 
 
-# GroupNorm statistics in the producing GEMM's epilogue: needs the activation-free ("lean") epilogue of mtgemm.cu, so
-# both switches travel together (environment overrides for A/B runs)
-# Off by default: measured neutral inside the step (groupnorm -0.5 ms, GEMM epilogues +3 ms on a power-capped B200,
-# profiles/r02_bench_newepi_gnfuse.json vs r02_bench_newepi.json); B200SVD_GN_FUSE=1 turns it on.
-GN_FUSE = (os.environ.get("B200SVD_GN_FUSE", "0") != "0" and os.environ.get("B200SVD_LEAN_EPI", "1") != "0")
+# GroupNorm statistics in the producing GEMM's epilogue (activation-free bf16 launches only).  Off by default;
+# B200SVD_GN_FUSE=1 turns it on.
+GN_FUSE = os.environ.get("B200SVD_GN_FUSE", "0") != "0"
 
 
 @lru_cache(maxsize=None)
@@ -209,8 +207,7 @@ def _gn_slots(m_ext, m_box, p):
     hi = z1 + z2 * e1 + z3 * e1 * e2
     if bool(((lo // p != hi // p) & ok).any()):
         return 0
-    m_tiles = t1 * t2 * t3
-    return (m_tiles + (m_tiles & 1)) * 4                         # pair tiles may decode one M tile past the end
+    return t1 * t2 * t3 * 4                                      # the GEMM writes every slot of every M tile
 
 
 def _gn_request(gn_rows, m_ext, m_box, n_out, act, out_fp32, device):
@@ -377,7 +374,7 @@ def small_attn(q, k, v, *, b, s, heads, lq, lk, kv_per_pixel=True, out=None):
     if out is None:
         out = torch.empty((b * lq * s, Cc), dtype=torch.bfloat16, device=q.device)
     if kv_per_pixel and all(t.data_ptr() % 16 == 0 for t in (q, k, v)):
-        # tensor-core path: 4 pixels x 32 padded frames per tcgen05 tile
+        # tensor-core path: 4 pixels x 32 padded frames per CTA, wgmma tiles
         _call("b200svd_pixel_attn", _ptr(q), q.stride(0), _ptr(k), k.stride(0), _ptr(v), v.stride(0), _ptr(out),
               out.stride(0), b, s, heads, lq, lk, 64 ** -0.5, _stream(),
               flops=4.0 * b * s * heads * lq * lk * 64, nbytes=2.0 * Cc * (2 * b * lq * s + 2 * b * lk * s),

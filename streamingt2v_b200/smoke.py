@@ -8,7 +8,7 @@ import torch
 
 def run_smoke():
     if not torch.cuda.is_available():
-        raise RuntimeError("smoke() needs a CUDA device (B200)")
+        raise RuntimeError("smoke() needs a CUDA device (H100)")
     from oracle import streaming_svd_oracle as orc  # checker only
     from . import arch, ops, synth
     from .wrapper import B200StreamingWrapper

@@ -1,4 +1,4 @@
-"""Stage driver of the autoregressive StreamingSVD stage (SURVEY.md section 8 row a22) on top of the B200 pieces:
+"""Stage driver of the autoregressive StreamingSVD stage (SURVEY.md section 8 row a22) on top of the project's pieces:
 denoiser seam (`B200StreamingWrapper`), sampler (`B200EulerEDMSampler`) and temporal VAE decoder (`B200VaeDecoder`).
 
 Mirrors, method for method, the reference's `StreamingSVD` LightningModule

@@ -1,4 +1,4 @@
-"""Temporal VAE decoder on the B200 kernels — drop-in for `first_stage_model.decode(z, timesteps=n)`
+"""Temporal VAE decoder on the project's kernels — drop-in for `first_stage_model.decode(z, timesteps=n)`
 (reference code/models/svd/sgm/models/autoencoder.py:210-212 -> VideoDecoder, temporal_ae.py:291-347; call site
 code/diffusion_trainer/streaming_svd.py:143).  Same conventions as model.py: channel-last bf16 rows, every tensor op
 is one of our kernels, fp32 accumulation (the reference runs this stage in fp32; tolerance in DESIGN.md)."""
@@ -118,7 +118,7 @@ class B200VaeDecoder:
 
 
 class B200VaeEncoder:
-    """SD-VAE encoder of the conditioner on the B200 kernels — drop-in for `AutoencoderKLModeOnly.encode(x)`
+    """SD-VAE encoder of the conditioner on the project's kernels — drop-in for `AutoencoderKLModeOnly.encode(x)`
     (reference code/models/svd/sgm/models/autoencoder.py:468-473,602-615 -> Encoder, diffusionmodules/model.py:487-601;
     called once per chunk by VideoPredictionEmbedderWithEncoder, encoders/modules.py:697-729): returns the posterior
     MODE [n, 4, H/8, W/8] (the caller applies its scale factor, as the reference embedder does).  Same conventions as

@@ -22,7 +22,7 @@ class B200StreamingWrapper(nn.Module):
                  device="cuda:0"):
         super().__init__()
         if not torch.cuda.is_available():
-            raise RuntimeError("B200StreamingWrapper needs a CUDA device (sm_100a); there is no CPU fallback")
+            raise RuntimeError("B200StreamingWrapper needs a CUDA device (sm_90a); there is no CPU fallback")
         self.cfg = cfg
         self.num_frame_conditioning = cfg.num_frame_conditioning
         self.engine = B200Denoiser(cfg, sd_unet, sd_ctrl, device)

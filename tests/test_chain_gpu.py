@@ -1,4 +1,4 @@
-"""The whole sampling chain of one StreamingSVD chunk on the B200 path — B200EulerEDMSampler x B200StreamingWrapper
+"""The whole sampling chain of one StreamingSVD chunk on the project's GPU path — B200EulerEDMSampler x B200StreamingWrapper
 x B200VaeDecoder — against the golden produced by the UNMODIFIED reference classes (EulerEDMSampler + Denoiser +
 StreamingWrapper + VideoDecoder, oracle/make_golden_chain.py) on identical noise, conditioning and weights.
 

@@ -3,7 +3,7 @@
 Checked against (1) the committed golden vectors produced by the UNMODIFIED reference modules (tests/golden,
 oracle/make_golden.py) and (2) the CPU oracle on the same seeded inputs, tap by tap.
 Tolerance (bf16 activations + fp32 accumulate, vs the reference's fp32 CPU result): relative L2 <= 3e-2 on the
-output latent update and on every block output; max-abs <= 6e-2 * max|ref|.  Measured on B200: see profiles/.
+output latent update and on every block output; max-abs <= 6e-2 * max|ref|.
 """
 import dataclasses
 import os
@@ -50,17 +50,19 @@ def test_streaming_wrapper_vs_reference_golden(cuda_dev, name, apm):
     out = out.float().cpu()
     assert torch.isfinite(out).all()
     ref = torch.from_numpy(g["out"])
+    hstep = int(g["out_hstep"][0]) if "out_hstep" in g else 1  # large goldens keep every hstep-th latent row
+    out = out[:, :, ::hstep]
     r = _rel(out, ref)
     mx = (out - ref).abs().max().item()
     print(f"[{name}] out vs REFERENCE golden: rel_l2={r:.4e} max_abs={mx:.4e} ref_absmax={ref.abs().max():.3f}")
     # second call (exercises the cached conditioning path) must reproduce the first bit for bit
-    out2 = m(xd, td, cd, **kwd).float().cpu()
+    out2 = m(xd, td, cd, **kwd).float().cpu()[:, :, ::hstep]
     assert torch.equal(out, out2), "non-deterministic / stale cached conditioning"
     # tap-by-tap against the oracle
     taps = {}
     with torch.no_grad():
         o_ref = orc.streaming_wrapper_forward(sd_u, sd_c, cfg, x, t, c, taps=taps, **kw)
-    assert _rel(o_ref, ref) < 1e-4  # the oracle itself reproduces the reference's golden output
+    assert _rel(o_ref[:, :, ::hstep], ref) < 1e-4  # the oracle itself reproduces the reference's golden output
     worst = 0.0
     for tname, (tt, n, hh, ww) in m.engine.debug_taps.items():
         if tname in taps:

@@ -27,7 +27,7 @@ def _rand(shape, dev, scale=1.0, seed=0):
 
 @pytest.fixture(params=[3, 4, 5], ids=["two-pass", "single-pass", "16-warp"])
 def fa_variant(request, cuda_dev):
-    """Every FlashAttention case runs with each softmax organisation of the kernel (b200svd_flash_attn_variant)."""
+    """Every FlashAttention case runs under each softmax variant the ABI accepts (the sm_90 kernel has one organisation)."""
     from streamingt2v_b200 import ops
     prev = ops.flash_attn_variant(request.param)
     yield request.param

@@ -1,6 +1,5 @@
-"""CPU: the built sm_100a library really contains what DESIGN.md says it does — checked on the SASS of
-streamingt2v_b200/libb200svd.so with cuobjdump (mnemonics per /opt/skills/guides/B200_PROFILING.md: tcgen05.mma ->
-UTCHMMA, tcgen05.ld/st -> LDTM/STTM, TMA -> UTMALDG/UTMASTG, tcgen05.commit -> UTCBAR, cluster barrier -> UCGABAR).
+"""CPU: the built sm_90a library really contains what DESIGN.md says it does — checked on the SASS of
+streamingt2v_b200/libb200svd.so with cuobjdump (wgmma -> HGMMA, TMA load -> UTMALDG, setmaxnreg -> USETMAXREG).
 Skipped when cuobjdump is not on the PATH."""
 import re
 import shutil
@@ -35,48 +34,25 @@ def _of(sass, needle):
     return sel
 
 
-def test_arch_is_sm100a(sass):
-    import subprocess
+def test_arch_is_sm90a(sass):
     from streamingt2v_b200 import _lib
     out = subprocess.run(["cuobjdump", "-lelf", str(_lib.lib_path())], capture_output=True, text=True).stdout
-    assert "sm_100a" in out
+    assert "sm_90a" in out
 
 
-def test_gemm_uses_tcgen05_tma_and_2sm(sass):
+def test_gemm_uses_wgmma_and_tma(sass):
     g = _of(sass, "mtgemm_kernel")
+    assert len(g) == 5, sorted(g)                                          # N tiles 32, 64, 128, 160, 256
     for name, body in g.items():
-        assert "UTCHMMA" in body, f"{name}: no tcgen05.mma"
-        assert "UTMALDG" in body and "UTMASTG" in body, f"{name}: TMA load/store missing"
-        assert "LDTM" in body, f"{name}: no tcgen05.ld (TMEM epilogue)"
-        assert not re.search(r"(?<![A-Z])(HMMA|WGMMA|HGMMA)\b", body), f"{name}: legacy (mma.sync / wgmma) path"
-    pair = {k: v for k, v in g.items() if "UTCHMMA.2CTA" in v}
-    assert len(pair) >= 2, "no cta_group::2 instantiation"              # <160,2>, <256,2> (+ cluster-of-4 variants)
-    assert all("UTMALDG.5D.2CTA" in v or "UTMALDG.5D.MULTICAST.2CTA" in v for v in pair.values())
-    assert all("UCGABAR" in v for v in pair.values())                    # cluster barrier around the pair's lifetime
+        assert "HGMMA" in body, f"{name}: no wgmma"
+        assert "UTMALDG" in body, f"{name}: TMA load missing"
+        assert "USETMAXREG" in body, f"{name}: producer / consumer register split missing"
+        assert not re.search(r"(?<![A-Z])HMMA\b", body), f"{name}: legacy mma.sync path"
 
 
-def test_attention_kernels_use_tcgen05(sass):
+def test_attention_kernels_use_wgmma(sass):
     for needle in ("flash_attn_kernel", "pixel_attn_kernel"):
         for name, body in _of(sass, needle).items():
-            assert "UTCHMMA" in body and "UTMALDG" in body, f"{name}: not on tcgen05 + TMA"
-            assert "LDTM" in body and "STTM" in body, f"{name}: P/O should move through TMEM"
+            assert "HGMMA" in body and "UTMALDG" in body, f"{name}: not on wgmma + TMA"
             assert "MUFU.EX2" in body
-
-
-def test_round2_epilogues_and_softmax_use_packed_math(sass):
-    """The specialised GEGLU / lean epilogues (mtgemm EPI = 1 / 2) and the single-pass softmax compute on packed fp32 pairs
-    (FFMA2 / FMUL2 / FADD2) and the softmax max on FMNMX3; the 320-wide 2-SM tile exists; the softmax warps re-split the
-    register file (setmaxnreg -> USETMAXREG)."""
-    geglu = {k: v for k, v in _of(sass, "mtgemm_kernel").items() if "ILi256ELi2ELi1E" in k or "ILi256ELi1ELi1E" in k}
-    assert len(geglu) == 2, sorted(geglu)
-    for name, body in geglu.items():
-        assert body.count("FFMA2") >= 100 and "FMUL2" in body and "FADD2" in body, f"{name}: GEGLU epilogue is not packed"
-    lean = {k: v for k, v in _of(sass, "mtgemm_kernel").items() if k.endswith("ELi2EEEv14CUtensorMap_stS1_S1_S1_S1_S1_S1_NS_7GemmDevE")}
-    assert len(lean) >= 6 and all("FFMA2" in v or "FADD2" in v for v in lean.values())
-    assert any("ILi320ELi2E" in k for k in _of(sass, "mtgemm_kernel")), "320-wide 2-SM tile missing"
-    fast = {k: v for k, v in _of(sass, "flash_attn_kernel").items() if "Lb1E" in k}
-    assert fast, "single-pass softmax instantiation missing"
-    for name, body in fast.items():
-        assert "FMNMX3" in body and "FFMA2" in body and "FADD2" in body, f"{name}: softmax is not on packed math"
-    for name, body in {**_of(sass, "flash_attn_kernel"), **_of(sass, "flash_attn5_kernel")}.items():
-        assert "USETMAXREG" in body, f"{name}: no setmaxnreg"
+            assert not re.search(r"(?<![A-Z])HMMA\b", body), f"{name}: legacy mma.sync path"
