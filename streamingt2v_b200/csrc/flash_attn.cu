@@ -213,6 +213,10 @@ extern "C" int b200svd_flash_attn(const void* qkv, int64_t ldqkv, void* out, int
     set_error("flash_attn: leading dims must be multiples of 8");
     return 1;
   }
+  if ((reinterpret_cast<uintptr_t>(out) & 15) != 0) {  // the epilogue stores 4-byte words from a 16-byte base
+    set_error("flash_attn: out must be 16-byte aligned");
+    return 1;
+  }
   const int C = heads * FA_D;
   CUtensorMap tm;
   uint64_t dims[3] = {(uint64_t)3 * C, (uint64_t)s, (uint64_t)n};

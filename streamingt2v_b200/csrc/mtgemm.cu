@@ -497,10 +497,17 @@ extern "C" int b200svd_gemm(const b200svd_gemm_params* p, void* stream) {
   // wgmma takes N <= 256: a 320-wide tile is computed as two 160-wide tiles
   if (bn == 320) bn = 160;
   auto al16 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
-  const bool bf16_ok = p->ldo % 8 == 0 && al16(p->out) && (p->res1 == nullptr || (p->ld1 % 8 == 0 && al16(p->res1))) &&
-                       (p->res2 == nullptr || (p->ld2 % 8 == 0 && al16(p->res2)));
-  if (!p->out_fp32 && !bf16_ok) {
+  // The epilogue stores column pairs as one word (bf16x2 or float2) and loads residual pairs as one 32-bit word
+  // whenever the element offset from the base is even, so every base must be aligned to that word.
+  const bool res_ok = (p->res1 == nullptr || (p->ld1 % 8 == 0 && al16(p->res1))) &&
+                      (p->res2 == nullptr || (p->ld2 % 8 == 0 && al16(p->res2)));
+  const bool bf16_ok = p->ldo % 8 == 0 && al16(p->out);
+  if (!res_ok || (!p->out_fp32 && !bf16_ok)) {
     set_error("b200svd_gemm: bf16 outputs/residuals need 16-byte aligned bases and leading dims that are multiples of 8");
+    return 1;
+  }
+  if (p->out_fp32 && (reinterpret_cast<uintptr_t>(p->out) & 7) != 0) {
+    set_error("b200svd_gemm: an fp32 output needs an 8-byte aligned base");
     return 1;
   }
   const uint32_t n_out = p->act == B200SVD_ACT_GEGLU ? p->n / 2 : p->n;

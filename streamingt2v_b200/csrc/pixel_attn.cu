@@ -168,6 +168,12 @@ extern "C" int b200svd_pixel_attn(const void* q, int64_t ldq, const void* k, int
     set_error("pixel_attn: leading dims must be multiples of 8");
     return 1;
   }
+  for (const void* t : {q, k, v, static_cast<const void*>(o)}) {
+    if ((reinterpret_cast<uintptr_t>(t) & 15) != 0) {
+      set_error("pixel_attn: q/k/v/o must be 16-byte aligned");
+      return 1;
+    }
+  }
   const int C = heads * 64;
   CUtensorMap tmQ, tmK, tmV;
   if (encode_pixel_view(&tmQ, q, ldq, C, b, s, lq)) return 1;

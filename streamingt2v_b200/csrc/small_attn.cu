@@ -153,6 +153,12 @@ extern "C" int b200svd_small_attn(const void* q, int64_t ldq, const void* k, int
     set_error("small_attn: leading dims must be multiples of 8");
     return 1;
   }
+  for (const void* t : {q, k, v, static_cast<const void*>(o)}) {  // 16-byte cp.async and uint4 loads / stores
+    if ((reinterpret_cast<uintptr_t>(t) & 15) != 0) {
+      set_error("small_attn: q/k/v/o must be 16-byte aligned");
+      return 1;
+    }
+  }
   SmallAttnParams p;
   p.q = reinterpret_cast<const __nv_bfloat16*>(q);
   p.k = reinterpret_cast<const __nv_bfloat16*>(k);

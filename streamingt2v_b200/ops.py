@@ -367,13 +367,14 @@ def flash_attn(qkv, n, s, heads, out=None):
 
 
 def small_attn(q, k, v, *, b, s, heads, lq, lk, kv_per_pixel=True, out=None):
-    """q: rows (b, i<lq, s); k, v: rows (b, j<lk, s) or (b, j) when kv_per_pixel=False; head dim 64."""
+    """q: rows (b, i<lq, s); k, v: rows (b, j<lk, s) or (b, j) when kv_per_pixel=False; head dim 64.
+    q/k/v/out need 16-byte aligned bases and leading dims that are multiples of 8 (both kernels check)."""
     for t in (q, k, v):
         assert t.dtype == torch.bfloat16 and t.dim() == 2 and t.stride(1) == 1
     Cc = heads * 64
     if out is None:
         out = torch.empty((b * lq * s, Cc), dtype=torch.bfloat16, device=q.device)
-    if kv_per_pixel and all(t.data_ptr() % 16 == 0 for t in (q, k, v)):
+    if kv_per_pixel:
         # tensor-core path: 4 pixels x 32 padded frames per CTA, wgmma tiles
         _call("b200svd_pixel_attn", _ptr(q), q.stride(0), _ptr(k), k.stride(0), _ptr(v), v.stride(0), _ptr(out),
               out.stride(0), b, s, heads, lq, lk, 64 ** -0.5, _stream(),

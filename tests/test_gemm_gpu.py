@@ -49,8 +49,7 @@ def test_linear(cuda_dev, M, K, N, bn):
 @pytest.mark.parametrize("M,K,N,bn", [(1357, 1280, 1280, 256), (384, 640, 640, 160), (129, 1280, 512, 256),
                                       (128 * 149 * 2 + 5, 320, 320, 160), (5000, 1280, 1000, 256)])
 def test_wide_tiles_epilogue(cuda_dev, M, K, N, bn):
-    """160/256-wide tiles (CTA pairs in the 2sm run): odd M-tile counts, ragged N, several tiles per CTA, all
-    epilogue operands."""
+    """160/256-wide N tiles: odd M-tile counts, ragged N, several tiles per persistent CTA, all epilogue operands."""
     from streamingt2v_b200 import ops, packing
     rpf = 64
     x = _rand((M, K), cuda_dev, seed=1)
@@ -72,9 +71,9 @@ def test_wide_tiles_epilogue(cuda_dev, M, K, N, bn):
                                       (3000, 960, 960, 320), (4096, 2560, 1280, 0), (640, 320, 960, 0)])
 @pytest.mark.parametrize("operands", ["all", "bias", "none", "res1"])
 def test_lean_epilogue(cuda_dev, M, K, N, bn, operands):
-    """Activation-free launches take the specialised packed-math epilogue (mtgemm EPI = 2): bias, per-frame vector,
-    s_acc and both residuals in every combination the network uses; 128/160/256-wide tiles and the 320-wide 2-SM tile
-    (two N = 160 MMAs per k step, single-buffered accumulator), ragged M / N edges, several tiles per CTA."""
+    """Activation-free epilogues: bias, per-frame vector, s_acc and both residuals in every combination the network
+    uses; 128/160/256-wide tiles and bn = 320 (run as two 160-wide tiles, since wgmma takes N <= 256), ragged M / N
+    edges, several tiles per CTA."""
     from streamingt2v_b200 import ops, packing
     rpf = 64
     x = _rand((M, K), cuda_dev, seed=1)
@@ -103,7 +102,7 @@ def test_lean_epilogue(cuda_dev, M, K, N, bn, operands):
 
 @pytest.mark.parametrize("Nf,H,W,Cin,Cout", [(4, 24, 64, 320, 320), (3, 18, 32, 640, 640), (2, 36, 64, 960, 320)])
 def test_conv3x3_320_wide_tile(cuda_dev, monkeypatch, Nf, H, W, Cin, Cout):
-    """3x3 convolutions on the 320-wide 2-SM tile (forced), bias + residual, against F.conv2d."""
+    """3x3 convolutions with bn = 320 forced (run as 160-wide tiles), bias + residual, against F.conv2d."""
     from streamingt2v_b200 import ops, packing
     x = _rand((Nf, H, W, Cin), cuda_dev, seed=1)
     wt = _rand((Cout, Cin, 3, 3), cuda_dev, (9 * Cin) ** -0.5, seed=2)
@@ -164,17 +163,25 @@ def test_conv3x3(cuda_dev, N, H, W, Cin, Cout):
     _check(out, ref, f"conv3x3 N{N} {H}x{W} {Cin}->{Cout}")
 
 
+@pytest.mark.parametrize("pad_after_only", [False, True], ids=["pad1", "pad_after"])
 @pytest.mark.parametrize("N,H,W,Cin,Cout", [(2, 8, 8, 64, 64), (3, 18, 32, 128, 128), (2, 72, 128, 32, 96),
                                             (16, 4, 4, 64, 64), (1, 36, 64, 320, 320)])
-def test_conv3x3_s2(cuda_dev, N, H, W, Cin, Cout):
+def test_conv3x3_s2(cuda_dev, N, H, W, Cin, Cout, pad_after_only):
+    """pad_after_only=False: the UNet Downsample (pad 1 on every side); True: the autoencoder's Downsample (pad
+    (0, 1, 0, 1), then an unpadded conv)."""
     from streamingt2v_b200 import ops, packing
     x = _rand((N, H, W, Cin), cuda_dev, seed=1)
     w = _rand((Cout, Cin, 3, 3), cuda_dev, (9 * Cin) ** -0.5, seed=2)
     b = torch.randn(Cout, device=cuda_dev)
-    out = ops.conv3x3_s2(x, packing.pack_conv3x3(w, cuda_dev), b)
+    out = ops.conv3x3_s2(x, packing.pack_conv3x3(w, cuda_dev), b, pad_after_only=pad_after_only)
     torch.cuda.synchronize()
-    ref = F.conv2d(x.float().permute(0, 3, 1, 2), w.float(), b, padding=1, stride=2).permute(0, 2, 3, 1).reshape(-1, Cout)
-    _check(out, ref, f"conv3x3_s2 N{N} {H}x{W} {Cin}->{Cout}")
+    xf = x.float().permute(0, 3, 1, 2)
+    if pad_after_only:
+        ref = F.conv2d(F.pad(xf, (0, 1, 0, 1)), w.float(), b, stride=2)
+    else:
+        ref = F.conv2d(xf, w.float(), b, padding=1, stride=2)
+    ref = ref.permute(0, 2, 3, 1).reshape(-1, Cout)
+    _check(out, ref, f"conv3x3_s2 N{N} {H}x{W} {Cin}->{Cout} pad_after_only={pad_after_only}")
 
 
 @pytest.mark.parametrize("B,T,P,C", [(2, 8, 64, 64), (2, 25, 144, 128), (1, 7, 4, 256), (2, 25, 1024, 320)])

@@ -50,7 +50,7 @@ def test_flash_attn(cuda_dev, fa_variant, n, s, heads):
 @pytest.mark.parametrize("s,ramp", [(1024, 6.0), (2304, 3.0), (640, 12.0)])
 def test_flash_attn_rising_max(cuda_dev, fa_variant, s, ramp):
     """Key magnitudes grow along the sequence, so the row maxima keep rising by more than 2^8 between key blocks: the
-    single-pass softmax must take its redo path (rescale O and l, recompute P) and still match SDPA."""
+    online softmax must rescale O and l by the new maximum at nearly every block and still match SDPA."""
     from streamingt2v_b200 import ops
     n, heads = 2, 3
     Cc = heads * 64
