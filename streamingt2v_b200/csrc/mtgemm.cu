@@ -1,6 +1,7 @@
 // Multi-tap tensor-core GEMM for sm_90a.
 // TMA (rank-5 activation view) -> smem stage ring (128B swizzle) -> wgmma (fp32 accumulators in registers)
-// -> fused epilogue from registers.  See include/b200svd.h for the contract.
+// -> fused epilogue (bf16 outputs staged through shared memory and written by TMA stores).
+// See include/b200svd.h for the contract.
 //
 // Replaces, underneath StreamingWrapper.forward (reference code/models/diffusion/wrappers.py:23-78):
 //   nn.Linear            code/models/svd/sgm/modules/attention.py:94-120,262-351, video_attention.py:23-168
@@ -10,10 +11,12 @@
 //     residual / AlphaBlender diffusionmodules/util.py:358-370).
 //
 // Persistent CTAs (one per SM) walk the output tiles with a grid stride (N tile fastest).  Three warpgroups:
-//   warpgroup 0     TMA producer for A/B (one thread; the stage ring runs ahead across tiles, so the next tile's
-//                   operands stream in while the consumers run the epilogue of the current one)
+//   warpgroup 0     TMA producers: thread 0 loads A/B (the stage ring runs ahead across tiles, so the next tile's
+//                   operands stream in while the consumers run the epilogue of the current one); thread 32 loads the
+//                   residuals of bf16 outputs into their own ring
 //   warpgroups 1-2  consumers: each owns 64 rows of the 128-row tile, issues m64nBNk16 wgmma on the shared B stage
-//                   and applies the epilogue straight from its accumulator registers.
+//                   and applies the epilogue to its accumulator registers.  bf16 outputs are written 32 columns at a
+//                   time through a shared-memory staging buffer and a TMA store; fp32 outputs are stored directly.
 // A convolution tap is a shifted box of the same activation view, so taps and K blocks form one reduction loop.
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -57,6 +60,10 @@ struct GemmDev {
   int32_t* gn_slot_sample;
   int64_t gn_ld;
   uint32_t gn_rows;
+  int32_t staged;      // bf16 output through shared memory and TMA stores (else straight from registers)
+  uint32_t stages;     // depth of the A/B stage ring
+  uint32_t res_slots;  // depth of the residual ring (bf16 outputs with residuals, else 0)
+  uint32_t wg_off[3];  // row-box origin of the second consumer warpgroup's 64 rows (bf16 output stores)
 };
 
 constexpr int BM = 128;
@@ -64,23 +71,45 @@ constexpr int BK = 64;
 constexpr int A_STAGE_BYTES = BM * BK * 2;  // 16 KB
 constexpr int NUM_THREADS = 3 * 128;        // producer warpgroup + two consumer warpgroups
 constexpr int SMEM_LIMIT = 232448;          // 227 KB of dynamic shared memory per block
+constexpr int MAX_STAGES = 6;
+constexpr int MIN_STAGES = 3;
+// bf16 epilogue: the tile is processed in 32-column sub-tiles (64-byte rows, SWIZZLE_64B)
+constexpr int SUB_W = 32;
+constexpr int STG_SLOT_BYTES = 64 * SUB_W * 2;    // one warpgroup's 64 rows of one sub-tile: 4 KB
+constexpr int STG_SLOTS = 2;                      // staging buffers per consumer warpgroup
+constexpr int STG_BYTES = 2 * STG_SLOTS * STG_SLOT_BYTES;
+constexpr int RES_SLOT_BYTES = BM * SUB_W * 2;    // one residual sub-tile, both warpgroups: 8 KB
+constexpr int MAX_RES_SLOTS = 16;
+constexpr int GN_BYTES = 2 * 2 * 2 * SUB_W * 8;  // [warpgroup][buffer][quadrant][column][sum, sum of squares]
+constexpr int BAR_BYTES = 512;
+constexpr int FIXED_BYTES = STG_BYTES + GN_BYTES + BAR_BYTES;
+static_assert(2 * (MAX_STAGES + MAX_RES_SLOTS) * 8 <= BAR_BYTES, "barrier area");
 
+// Shared memory (offsets in bytes, every region 1024-byte aligned):
+//   [0, stages * STAGE_BYTES)   A/B stage ring
+//   res_slots * RES_SLOT_BYTES  residual ring (bf16 outputs with residuals)
+//   STG_BYTES                   output staging, per consumer warpgroup
+//   GN_BYTES                    GroupNorm partials of the partner warp
+//   BAR_BYTES                   mbarriers
+// The stage count and the residual ring are chosen per launch (launch<BN>): a launch with residuals trades A/B
+// stages (not below MIN_STAGES) for a residual ring that holds a whole tile's residuals where it fits.
 template <int BN>
 struct TileCfg {
   static constexpr int B_STAGE_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
-  static constexpr int GN_BYTES = 4 * BN * 8;  // per 32-row quadrant: (sum, sum of squares) per column
-  static constexpr int FIXED_BYTES = GN_BYTES + 256;
   static constexpr int STAGES_FIT = (SMEM_LIMIT - FIXED_BYTES) / STAGE_BYTES;
-  static constexpr int STAGES = STAGES_FIT > 6 ? 6 : STAGES_FIT;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + FIXED_BYTES;
+  static constexpr int STAGES = STAGES_FIT > MAX_STAGES ? MAX_STAGES : STAGES_FIT;
+  static constexpr int SUBTILES = BN / SUB_W;
   // accumulator registers per consumer thread: BN / 2; the 256-wide tile needs the producer's registers
   static constexpr int CONSUMER_REGS = BN > 128 ? 232 : 160;
   static constexpr int PRODUCER_REGS = 40;
-  static_assert(STAGES >= 3, "pipeline depth");
-  static_assert(SMEM_BYTES <= SMEM_LIMIT, "shared memory budget");
+  static constexpr int RES_SLOTS_AT_MIN = (SMEM_LIMIT - FIXED_BYTES - MIN_STAGES * STAGE_BYTES) / RES_SLOT_BYTES;
+  static int res_slots_fit(int stages) { return (SMEM_LIMIT - FIXED_BYTES - stages * STAGE_BYTES) / RES_SLOT_BYTES; }
+  static_assert(STAGES >= 4, "pipeline depth without residuals");
+  static_assert(RES_SLOTS_AT_MIN >= 2, "two residuals need two ring slots");
+  static_assert(STAGES * STAGE_BYTES + FIXED_BYTES <= SMEM_LIMIT, "shared memory budget");
   static_assert(STAGE_BYTES % 1024 == 0, "stage alignment");
-  static_assert(2 * (STAGES + 0) * 8 <= 256 - 8, "barrier area");
+  static_assert(BN % SUB_W == 0, "sub-tiles");
 };
 
 // `tile` enumerates (N tile fastest, then M tile).  An M tile decodes to the box origin of each of the three output
@@ -112,29 +141,62 @@ __device__ __forceinline__ void load_bf16_pair(const __nv_bfloat16* base, int64_
   }
 }
 
+// The epilogue arithmetic after bias and per-frame vector, shared by the fp32 and the bf16 output paths so that both
+// round the same fp32 value: activation (GEGLU: value * GELU(gate + gate bias), the gate bias already added), scale.
+// Multiplies and fused multiply-adds are written out so that the compiler cannot contract them differently.
+__device__ __forceinline__ float epi_act(const GemmDev& p, bool geglu, float v, float g) {
+  if (p.act == B200SVD_ACT_SILU) {
+    v = silu_fast(v);
+  } else if (p.act == B200SVD_ACT_GELU) {
+    v = gelu_fast(v);
+  } else if (geglu) {
+    v = __fmul_rn(v, gelu_fast(g));
+  }
+  return __fmul_rn(v, p.s_acc);
+}
+
+// byte offset of (row, 4-byte column pair `cp` of 16-byte chunk `ch`) in a 64-byte-row SWIZZLE_64B sub-tile buffer
+__device__ __forceinline__ uint32_t sw64_off(uint32_t row, uint32_t ch, uint32_t cp) {
+  return row * 64u + ((ch ^ ((row >> 1) & 3u)) << 4) + cp * 4u;
+}
+
 template <int BN>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
-mtgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmDev p) {
+mtgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+              const __grid_constant__ CUtensorMap tmO, const __grid_constant__ CUtensorMap tmR1,
+              const __grid_constant__ CUtensorMap tmR2, const GemmDev p) {
   using Cfg = TileCfg<BN>;
-  constexpr int STAGES = Cfg::STAGES;
   constexpr int R = BN / 2;  // accumulator registers per thread (m64nBN: 64 x BN over 128 threads)
   extern __shared__ __align__(1024) uint8_t smem[];  // SWIZZLE_128B operands need 1024-byte alignment
   if ((smem_u32(smem) & 1023u) != 0) __trap();
-  float* gn_x = reinterpret_cast<float*>(smem + STAGES * Cfg::STAGE_BYTES);  // [4 quadrants][BN][2]
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * Cfg::STAGE_BYTES + Cfg::GN_BYTES);
-  uint64_t* empty_bar = full_bar + STAGES;
+  const uint32_t stages = p.stages, rslots = p.res_slots;
+  uint8_t* res_smem = smem + stages * Cfg::STAGE_BYTES;
+  uint8_t* stg_smem = res_smem + rslots * RES_SLOT_BYTES;
+  float* gn_x = reinterpret_cast<float*>(stg_smem + STG_BYTES);  // [warpgroup][buffer][quadrant][32 columns][2]
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(stg_smem + STG_BYTES + GN_BYTES);
+  uint64_t* empty_bar = full_bar + MAX_STAGES;
+  uint64_t* res_full = empty_bar + MAX_STAGES;
+  uint64_t* res_empty = res_full + MAX_RES_SLOTS;
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int wg = warp >> 2;
   const uint32_t iters_per_tile = p.taps * p.kblocks;
+  const bool geglu = (p.act == B200SVD_ACT_GEGLU);
+  const uint32_t n_out = geglu ? p.n / 2 : p.n;
+  const uint32_t tile_out_w = geglu ? (uint32_t)BN / 2 : (uint32_t)BN;
 
   if (threadIdx.x == 0) {
     prefetch_tmap(&tmA);
     prefetch_tmap(&tmB);
-    for (int s = 0; s < STAGES; ++s) {
+    if (p.staged) prefetch_tmap(&tmO);
+    for (uint32_t s = 0; s < stages; ++s) {
       mbar_init(&full_bar[s], 1);
       mbar_init(&empty_bar[s], 2);  // one arrive per consumer warpgroup
+    }
+    for (uint32_t s = 0; s < rslots; ++s) {
+      mbar_init(&res_full[s], 1);
+      mbar_init(&res_empty[s], 2);
     }
     fence_barrier_init();
   }
@@ -144,7 +206,7 @@ mtgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
     asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(Cfg::PRODUCER_REGS));
     if (threadIdx.x == 0) {
       // ===================== TMA producer (A, B) =====================
-      uint32_t it = 0;
+      uint32_t st = 0, ph = 0;
       for (uint32_t tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
         uint32_t n_tile, mb1, mb2, mb3;
         decode_tile(p, tile, n_tile, mb1, mb2, mb3);
@@ -159,14 +221,41 @@ mtgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
           const int c2 = base[2] + p.tap_off[tap][2];
           const int c3 = base[3] + p.tap_off[tap][3];
           const int c4 = base[4] + p.tap_off[tap][4];
-          for (uint32_t kb = 0; kb < p.kblocks; ++kb, ++it) {
-            const uint32_t s = it % STAGES;
-            const uint32_t ph = (it / STAGES) & 1;
-            mbar_wait_parked(&empty_bar[s], ph ^ 1);
-            uint8_t* sa = smem + s * Cfg::STAGE_BYTES;
-            mbar_expect_tx(&full_bar[s], Cfg::STAGE_BYTES);
-            tma_load_5d(sa, &tmA, &full_bar[s], c0 + (int)(kb * BK), c1, c2, c3, c4);
-            tma_load_3d(sa + A_STAGE_BYTES, &tmB, &full_bar[s], (int)(kb * BK), n0, (int)tap);
+#pragma unroll 1
+          for (uint32_t kb = 0; kb < p.kblocks; ++kb) {
+            mbar_wait_parked(&empty_bar[st], ph ^ 1);
+            uint8_t* sa = smem + st * Cfg::STAGE_BYTES;
+            mbar_expect_tx(&full_bar[st], Cfg::STAGE_BYTES);
+            tma_load_5d(sa, &tmA, &full_bar[st], c0 + (int)(kb * BK), c1, c2, c3, c4);
+            tma_load_3d(sa + A_STAGE_BYTES, &tmB, &full_bar[st], (int)(kb * BK), n0, (int)tap);
+            if (++st == stages) {
+              st = 0;
+              ph ^= 1;
+            }
+          }
+        }
+      }
+    } else if (threadIdx.x == 32 && rslots != 0) {
+      // ============ TMA producer (residuals of bf16 outputs): sub-tile by sub-tile, res1 then res2 ============
+      // It runs ahead of the consumers by the depth of the ring, so a tile's residuals stream in during its MMAs.
+      if (p.res1 != nullptr) prefetch_tmap(&tmR1);
+      if (p.res2 != nullptr) prefetch_tmap(&tmR2);
+      uint32_t slot = 0, ph = 0;
+      for (uint32_t tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+        uint32_t n_tile, mb1, mb2, mb3;
+        decode_tile(p, tile, n_tile, mb1, mb2, mb3);
+        const uint32_t otile0 = n_tile * tile_out_w;
+        for (uint32_t c = 0; c < tile_out_w / SUB_W && otile0 + c * SUB_W < n_out; ++c) {
+          for (int r = 0; r < 2; ++r) {
+            if ((r == 0 ? p.res1 : p.res2) == nullptr) continue;
+            mbar_wait_parked(&res_empty[slot], ph ^ 1);
+            mbar_expect_tx(&res_full[slot], RES_SLOT_BYTES);
+            tma_load_4d(res_smem + slot * RES_SLOT_BYTES, r == 0 ? &tmR1 : &tmR2, &res_full[slot],
+                        (int)(otile0 + c * SUB_W), (int)mb1, (int)mb2, (int)mb3);
+            if (++slot == rslots) {
+              slot = 0;
+              ph ^= 1;
+            }
           }
         }
       }
@@ -179,25 +268,23 @@ mtgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
   const int cw = wg - 1;   // rows [64 cw, 64 cw + 64) of the tile
   const int wl = warp & 3;  // warp of the warpgroup: rows 16 wl .. 16 wl + 15 of those 64
   const int rq = lane >> 2, cq = lane & 3;
-  const bool geglu = (p.act == B200SVD_ACT_GEGLU);
-  const uint32_t n_out = geglu ? p.n / 2 : p.n;
-  const uint32_t tile_out_w = geglu ? (uint32_t)BN / 2 : (uint32_t)BN;
+  const bool leader = (threadIdx.x & 127) == 0;
   const uint32_t lb1 = p.m_lb[0], lb2 = p.m_lb[1];
   const int quad = 2 * cw + (wl >> 1);  // 32-row quadrant of the tile
   const bool gn = p.gn_part != nullptr;
   const bool gn_sender = (wl & 1) != 0;
-  const int gn_bar = 1 + quad;
-  float* gxq = gn_x + quad * BN * 2;
-  uint32_t it = 0;
+  uint32_t st = 0, sph = 0;         // A/B ring position
+  uint32_t rslot = 0, rph = 0;      // residual ring position
+  uint32_t stg_it = 0;              // sub-tiles staged by this warpgroup so far
   float acc[R];
 
   for (uint32_t tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
 #pragma unroll
     for (int i = 0; i < R; ++i) acc[i] = 0.f;
-    for (uint32_t i = 0; i < iters_per_tile; ++i, ++it) {
-      const uint32_t s = it % STAGES;
-      mbar_wait(&full_bar[s], (it / STAGES) & 1);
-      const uint32_t sa = smem_u32(smem + s * Cfg::STAGE_BYTES);
+    uint32_t prev = 0;
+    for (uint32_t i = 0; i < iters_per_tile; ++i) {
+      mbar_wait(&full_bar[st], sph);
+      const uint32_t sa = smem_u32(smem + st * Cfg::STAGE_BYTES);
       const uint64_t adesc = smem_desc_k_sw128(sa + cw * (A_STAGE_BYTES / 2));
       const uint64_t bdesc = smem_desc_k_sw128(sa + A_STAGE_BYTES);
       wgmma_fence_regs(acc);
@@ -209,11 +296,16 @@ mtgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
       wgmma_fence_regs(acc);
       // the MMAs of the previous stage have completed: hand it back to the producer
       wgmma_wait<1>();
-      if (i > 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[(it - 1) % STAGES]);
+      if (i > 0 && leader) mbar_arrive(&empty_bar[prev]);
+      prev = st;
+      if (++st == stages) {
+        st = 0;
+        sph ^= 1;
+      }
     }
     wgmma_wait<0>();
     wgmma_fence_regs(acc);
-    if ((threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[(it - 1) % STAGES]);
+    if (leader) mbar_arrive(&empty_bar[prev]);
 
     // ----- epilogue: thread holds rows r0 and r0 + 8, columns 8 j + 2 cq + {0, 1} (acc[4 j + 2 h + e]) -----
     uint32_t n_tile, mb1, mb2, mb3;
@@ -235,13 +327,160 @@ mtgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
                                               : nullptr;
     }
     constexpr int NJ = BN / 8;
+    if (p.staged) {
+      // ----- bf16 output: 32-column sub-tiles staged in shared memory (SWIZZLE_64B, conflict-free fragment
+      // writes), written by one TMA store per warpgroup and sub-tile; residuals come from the TMA-fed ring -----
+#pragma unroll
+      for (int c = 0; c < Cfg::SUBTILES; ++c) {
+        if (geglu && c >= Cfg::SUBTILES / 2) break;  // gate columns are consumed with their value columns
+        if (otile0 + (uint32_t)(c * SUB_W) >= n_out) break;
+        uint8_t* stg = stg_smem + (cw * STG_SLOTS + (stg_it & 1)) * STG_SLOT_BYTES;
+        float* gxb = gn_x + ((cw * 2 + (stg_it & 1)) * 2 + (wl >> 1)) * (SUB_W * 2);
+        // residual sub-tiles of this warpgroup's 64 rows, in the order the residual producer loads them
+        const uint8_t* r1s = nullptr;
+        const uint8_t* r2s = nullptr;
+        uint32_t r1slot = 0, r2slot = 0;
+        if (p.res1 != nullptr) {
+          r1slot = rslot;
+          mbar_wait(&res_full[rslot], rph);
+          r1s = res_smem + rslot * RES_SLOT_BYTES + cw * STG_SLOT_BYTES;
+          if (++rslot == rslots) {
+            rslot = 0;
+            rph ^= 1;
+          }
+        }
+        if (p.res2 != nullptr) {
+          r2slot = rslot;
+          mbar_wait(&res_full[rslot], rph);
+          r2s = res_smem + rslot * RES_SLOT_BYTES + cw * STG_SLOT_BYTES;
+          if (++rslot == rslots) {
+            rslot = 0;
+            rph ^= 1;
+          }
+        }
+#pragma unroll
+        for (int jj = 0; jj < 4; ++jj) {
+          const int j = 4 * c + jj;
+          const uint32_t tcol = (uint32_t)(8 * j + 2 * cq);
+          const uint32_t ocol = otile0 + tcol;
+          const bool in0 = ocol < n_out, in1 = ocol + 1 < n_out;
+          float gs0 = 0.f, gs1 = 0.f, gq0 = 0.f, gq1 = 0.f;  // GroupNorm partials of the two columns
+          // bias, gate bias and per-frame values of the column pair, loaded together ahead of the arithmetic
+          float bv[2], gbv[2], fvv[2][2];
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const bool in = e == 0 ? in0 : in1;
+            bv[e] = (p.bias != nullptr && in) ? __ldg(p.bias + n0 + tcol + e) : 0.f;
+            gbv[e] = (geglu && p.bias != nullptr) ? __ldg(p.bias + n0 + BN / 2 + tcol + e) : 0.f;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) fvv[h][e] = (fv[h] != nullptr && in) ? __ldg(fv[h] + ocol + e) : 0.f;
+          }
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const uint32_t off = sw64_off((uint32_t)(16 * wl + rq + 8 * h), (uint32_t)jj, (uint32_t)cq);
+            float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+            float g0 = 0.f, g1 = 0.f;
+            if (p.bias != nullptr) {
+              v0 += bv[0];
+              v1 += bv[1];
+            }
+            if (fv[h] != nullptr) {
+              v0 += fvv[h][0];
+              v1 += fvv[h][1];
+            }
+            if (geglu) {
+              g0 = acc[4 * (j + NJ / 2) + 2 * h];
+              g1 = acc[4 * (j + NJ / 2) + 2 * h + 1];
+              if (p.bias != nullptr) {
+                g0 += gbv[0];
+                g1 += gbv[1];
+              }
+            }
+            v0 = epi_act(p, geglu, v0, g0);
+            v1 = epi_act(p, geglu, v1, g1);
+            if (r1s != nullptr) {
+              const uint32_t w = *reinterpret_cast<const uint32_t*>(r1s + off);
+              v0 = __fmaf_rn(p.s1, bf16_lo(w), v0);
+              v1 = __fmaf_rn(p.s1, bf16_hi(w), v1);
+            }
+            if (r2s != nullptr) {
+              const uint32_t w = *reinterpret_cast<const uint32_t*>(r2s + off);
+              v0 = __fmaf_rn(p.s2, bf16_lo(w), v0);
+              v1 = __fmaf_rn(p.s2, bf16_hi(w), v1);
+            }
+            const uint32_t w = pack_bf16x2(v0, v1);
+            *reinterpret_cast<uint32_t*>(stg + off) = w;
+            if (gn && valid[h] && in0) {
+              // statistics of the bf16-ROUNDED values, the ones the consumer reads
+              const float r0 = bf16_lo(w), r1 = in1 ? bf16_hi(w) : 0.f;
+              gs0 += r0;
+              gs1 += r1;
+              gq0 = __fmaf_rn(r0, r0, gq0);
+              gq1 = __fmaf_rn(r1, r1, gq1);
+            }
+          }
+          if (gn) {
+            // column sums over the warp's 16 rows (lanes of equal cq), then over the quadrant's two warps via smem
+#pragma unroll
+            for (int o = 4; o < 32; o <<= 1) {
+              gs0 += __shfl_xor_sync(0xffffffffu, gs0, o);
+              gs1 += __shfl_xor_sync(0xffffffffu, gs1, o);
+              gq0 += __shfl_xor_sync(0xffffffffu, gq0, o);
+              gq1 += __shfl_xor_sync(0xffffffffu, gq1, o);
+            }
+            if (gn_sender && rq == 0)
+              *reinterpret_cast<float4*>(gxb + 2 * (8 * jj + 2 * cq)) = make_float4(gs0, gq0, gs1, gq1);
+            if (!gn_sender) {
+              acc[4 * j] = gs0;  // the accumulators of this column block are consumed: park the partials there
+              acc[4 * j + 1] = gq0;
+              acc[4 * j + 2] = gs1;
+              acc[4 * j + 3] = gq1;
+            }
+          }
+        }
+        fence_proxy_async_smem();  // the staged values are read by the TMA store (async proxy)
+        // the store issued one sub-tile ago has read the other staging buffer: it may be refilled next sub-tile
+        if (leader) tma_store_wait_read0();
+        named_bar_sync(5 + cw, 128);
+        if (leader) {
+          if (r1s != nullptr) mbar_arrive(&res_empty[r1slot]);
+          if (r2s != nullptr) mbar_arrive(&res_empty[r2slot]);
+          // the warpgroup's 64 rows: the tile's row box halved in its outermost non-unit dimension
+          tma_store_4d(&tmO, stg, (int)(otile0 + c * SUB_W), (int)(mb1 + (cw ? p.wg_off[0] : 0u)),
+                       (int)(mb2 + (cw ? p.wg_off[1] : 0u)), (int)(mb3 + (cw ? p.wg_off[2] : 0u)));
+          tma_store_commit();
+        }
+        if (gn && !gn_sender && rq == 0) {
+          const uint32_t slot = (tile / p.n_tiles) * 4u + (uint32_t)quad;
+          float2* dst = reinterpret_cast<float2*>(p.gn_part) + (int64_t)slot * p.gn_ld;
+#pragma unroll
+          for (int jj = 0; jj < 4; ++jj) {
+            const int j = 4 * c + jj;
+            const uint32_t ocol = otile0 + (uint32_t)(8 * j + 2 * cq);
+            if (ocol < n_out) {
+              const float4 o = *reinterpret_cast<const float4*>(gxb + 2 * (8 * jj + 2 * cq));
+              dst[ocol] = make_float2(acc[4 * j] + o.x, acc[4 * j + 1] + o.y);
+              if (ocol + 1 < n_out) dst[ocol + 1] = make_float2(acc[4 * j + 2] + o.z, acc[4 * j + 3] + o.w);
+            }
+          }
+        }
+        ++stg_it;
+      }
+      if (gn && !gn_sender && lane == 0 && n_tile == 0) {
+        // lane 0 holds the first row of the quadrant: if it is out of range, so is every row of the quadrant
+        const uint32_t slot = (tile / p.n_tiles) * 4u + (uint32_t)quad;
+        p.gn_slot_sample[slot] = valid[0] ? (int32_t)((uint32_t)row[0] / p.gn_rows) : -1;
+      }
+      continue;
+    }
+    // ----- fp32 output (pitches a tensor map cannot describe), or a bf16 output whose width is not a whole number
+    // of 16-byte chunks (a TMA store writes whole chunks): straight from the accumulator registers -----
 #pragma unroll
     for (int j = 0; j < NJ; ++j) {
       if (geglu && j >= NJ / 2) break;  // gate columns are consumed with their value columns
       const uint32_t tcol = 8 * j + 2 * cq;  // column in the tile (value column for GEGLU)
       const uint32_t ocol = otile0 + tcol;
       const bool in0 = ocol < n_out, in1 = ocol + 1 < n_out;
-      float gs0 = 0.f, gs1 = 0.f, gq0 = 0.f, gq1 = 0.f;  // GroupNorm partials of the two columns
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
@@ -254,34 +493,28 @@ mtgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
           v0 += __ldg(fv[h] + ocol);
           if (in1) v1 += __ldg(fv[h] + ocol + 1);
         }
-        if (p.act == B200SVD_ACT_SILU) {
-          v0 = silu_fast(v0);
-          v1 = silu_fast(v1);
-        } else if (p.act == B200SVD_ACT_GELU) {
-          v0 = gelu_fast(v0);
-          v1 = gelu_fast(v1);
-        } else if (geglu) {
-          float g0 = acc[4 * (j + NJ / 2) + 2 * h], g1 = acc[4 * (j + NJ / 2) + 2 * h + 1];
+        float g0 = 0.f, g1 = 0.f;
+        if (geglu) {
+          g0 = acc[4 * (j + NJ / 2) + 2 * h];
+          g1 = acc[4 * (j + NJ / 2) + 2 * h + 1];
           if (p.bias != nullptr) {
             g0 += __ldg(p.bias + n0 + BN / 2 + tcol);
             if (in1) g1 += __ldg(p.bias + n0 + BN / 2 + tcol + 1);
           }
-          v0 *= gelu_fast(g0);
-          v1 *= gelu_fast(g1);
         }
-        v0 *= p.s_acc;
-        v1 *= p.s_acc;
+        v0 = epi_act(p, geglu, v0, g0);
+        v1 = epi_act(p, geglu, v1, g1);
         if (p.res1 != nullptr) {
           float a, b;
           load_bf16_pair(p.res1, row[h] * p.ld1 + ocol, in1, a, b);
-          v0 += p.s1 * a;
-          v1 += p.s1 * b;
+          v0 = __fmaf_rn(p.s1, a, v0);
+          v1 = __fmaf_rn(p.s1, b, v1);
         }
         if (p.res2 != nullptr) {
           float a, b;
           load_bf16_pair(p.res2, row[h] * p.ld2 + ocol, in1, a, b);
-          v0 += p.s2 * a;
-          v1 += p.s2 * b;
+          v0 = __fmaf_rn(p.s2, a, v0);
+          v1 = __fmaf_rn(p.s2, b, v1);
         }
         if (p.out_fp32) {
           float* op = reinterpret_cast<float*>(p.out) + row[h] * p.ldo + ocol;
@@ -293,62 +526,16 @@ mtgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
           }
         } else {
           __nv_bfloat16* op = reinterpret_cast<__nv_bfloat16*>(p.out) + row[h] * p.ldo + ocol;
-          const uint32_t w = pack_bf16x2(v0, v1);
           if (in1) {
-            *reinterpret_cast<uint32_t*>(op) = w;  // ldo % 8 == 0 and an even column: 4-byte aligned
+            *reinterpret_cast<uint32_t*>(op) = pack_bf16x2(v0, v1);  // ldo % 8 == 0 and an even column: 4-byte aligned
           } else {
             op[0] = __float2bfloat16(v0);
           }
-          // statistics of the bf16-ROUNDED values, the ones the consumer reads
-          const float r0 = bf16_lo(w), r1 = in1 ? bf16_hi(w) : 0.f;
-          gs0 += r0;
-          gs1 += r1;
-          gq0 += r0 * r0;
-          gq1 += r1 * r1;
         }
       }
-      if (gn) {
-        // column sums over the warp's 16 rows (lanes of equal cq), then over the quadrant's two warps via smem
-#pragma unroll
-        for (int o = 4; o < 32; o <<= 1) {
-          gs0 += __shfl_xor_sync(0xffffffffu, gs0, o);
-          gs1 += __shfl_xor_sync(0xffffffffu, gs1, o);
-          gq0 += __shfl_xor_sync(0xffffffffu, gq0, o);
-          gq1 += __shfl_xor_sync(0xffffffffu, gq1, o);
-        }
-        if (gn_sender && rq == 0)
-          *reinterpret_cast<float4*>(gxq + 2 * tcol) = make_float4(gs0, gq0, gs1, gq1);
-        if (!gn_sender) {
-          acc[4 * j] = gs0;  // the accumulators of this column block are consumed: park the partials there
-          acc[4 * j + 1] = gq0;
-          acc[4 * j + 2] = gs1;
-          acc[4 * j + 3] = gq1;
-        }
-      }
-    }
-    if (gn) {
-      named_bar_sync(gn_bar, 64);  // the partner warp's partials are in shared memory
-      if (!gn_sender) {
-        const uint32_t slot = (tile / p.n_tiles) * 4u + (uint32_t)quad;
-        if (rq == 0) {
-          float2* dst = reinterpret_cast<float2*>(p.gn_part) + (int64_t)slot * p.gn_ld;
-#pragma unroll
-          for (int j = 0; j < NJ; ++j) {
-            const uint32_t tcol = 8 * j + 2 * cq;
-            const uint32_t ocol = otile0 + tcol;
-            if (ocol < n_out) {
-              const float4 o = *reinterpret_cast<const float4*>(gxq + 2 * tcol);
-              dst[ocol] = make_float2(acc[4 * j] + o.x, acc[4 * j + 1] + o.y);
-              if (ocol + 1 < n_out) dst[ocol + 1] = make_float2(acc[4 * j + 2] + o.z, acc[4 * j + 3] + o.w);
-            }
-          }
-        }
-        // lane 0 holds the first row of the quadrant: if it is out of range, so is every row of the quadrant
-        if (lane == 0 && n_tile == 0) p.gn_slot_sample[slot] = valid[0] ? (int32_t)((uint32_t)row[0] / p.gn_rows) : -1;
-      }
-      named_bar_sync(gn_bar, 64);  // read before the next tile overwrites
     }
   }
+  if (p.staged && leader) tma_store_wait_all();  // shared memory must outlive the last stores' reads
 }
 
 static int ilog2_exact(uint32_t v) {
@@ -358,8 +545,16 @@ static int ilog2_exact(uint32_t v) {
   return l;
 }
 
+// Tensor maps of the bf16 epilogue: the output, res1 and res2 as (n_out, m1, m2, m3) views with row strides
+// out_rs[i] * leading dimension, and a 32-column box (SWIZZLE_64B).  Hardware clipping handles ragged M in each of
+// the three row dimensions, the N edge and column slices of wider buffers.
+struct EpiMaps {
+  CUtensorMap out, res1, res2;
+};
+
 template <int BN>
-static int launch(const b200svd_gemm_params* p, const CUtensorMap& tmA, const GemmDev& d, cudaStream_t st) {
+static int launch(const b200svd_gemm_params* p, const CUtensorMap& tmA, const EpiMaps& em, const GemmDev& d,
+                  cudaStream_t st) {
   using Cfg = TileCfg<BN>;
   // weights [taps][n][k] -> TMA dims (k, n, taps)
   CUtensorMap tmB;
@@ -369,10 +564,25 @@ static int launch(const b200svd_gemm_params* p, const CUtensorMap& tmA, const Ge
   if (encode_tmap_bf16(&tmB, p->w_ptr, 3, bd, bs, bb)) return 1;
   GemmDev dd = d;
   dd.n_tiles = (p->n + BN - 1) / BN;
+  // Ring depths.  Without residuals every byte past the fixed areas goes to A/B stages.  With residuals (bf16
+  // output) stages are given up, down to MIN_STAGES, until the residual ring holds a whole tile's residual sub-tiles.
+  int stages = Cfg::STAGES, res_slots = 0;
+  const int nres = d.staged ? (p->res1 != nullptr) + (p->res2 != nullptr) : 0;
+  if (nres > 0) {
+    const int tile_out_w = p->act == B200SVD_ACT_GEGLU ? BN / 2 : BN;
+    int want = nres * (tile_out_w / SUB_W);
+    if (want > MAX_RES_SLOTS) want = MAX_RES_SLOTS;
+    while (stages > MIN_STAGES && Cfg::res_slots_fit(stages) < want) --stages;
+    res_slots = Cfg::res_slots_fit(stages);
+    if (res_slots > want) res_slots = want;
+  }
+  dd.stages = (uint32_t)stages;
+  dd.res_slots = (uint32_t)res_slots;
+  const int smem_bytes = stages * Cfg::STAGE_BYTES + res_slots * RES_SLOT_BYTES + FIXED_BYTES;
   const int slot = dev_slot();
   static bool attr_set[B200_MAX_DEVICES] = {};
   if (!attr_set[slot]) {
-    cudaError_t e = cudaFuncSetAttribute(mtgemm_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
+    cudaError_t e = cudaFuncSetAttribute(mtgemm_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT);
     if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(mtgemm)");
     attr_set[slot] = true;
   }
@@ -384,7 +594,7 @@ static int launch(const b200svd_gemm_params* p, const CUtensorMap& tmA, const Ge
   }
   dd.total_tiles = (uint32_t)total;
   const uint32_t grid = (uint32_t)(total < (uint64_t)sm_count() ? total : (uint64_t)sm_count());
-  mtgemm_kernel<BN><<<grid, NUM_THREADS, Cfg::SMEM_BYTES, st>>>(tmA, tmB, dd);
+  mtgemm_kernel<BN><<<grid, NUM_THREADS, smem_bytes, st>>>(tmA, tmB, em.out, em.res1, em.res2, dd);
   B200_CHECK_LAUNCH("mtgemm launch");
   return 0;
 }
@@ -519,15 +729,51 @@ extern "C" int b200svd_gemm(const b200svd_gemm_params* p, void* stream) {
     return 1;
   }
 
+  // bf16 outputs are staged in shared memory and written by TMA stores, their residuals read by TMA loads.  A TMA
+  // store writes whole 16-byte chunks of a row, so this needs an output width that is a multiple of 8.
+  EpiMaps em;
+  memset(&em, 0, sizeof(em));
+  d.staged = !p->out_fp32 && n_out % 8 == 0;
+  if (d.staged) {
+    for (int i = 0; i < 3; ++i) {
+      if (p->out_rs[i] <= 0) {
+        set_error("b200svd_gemm: a bf16 output needs positive row strides, got out_rs[%d]=%lld", i,
+                  (long long)p->out_rs[i]);
+        return 1;
+      }
+    }
+    const uint64_t od[4] = {n_out, p->m_ext[0], p->m_ext[1], p->m_ext[2]};
+    auto row_strides = [&](int64_t ld, uint64_t* s) {
+      for (int i = 0; i < 3; ++i) s[i] = (uint64_t)p->out_rs[i] * (uint64_t)ld * 2;
+    };
+    // each consumer warpgroup stores its 64 rows: the row box halved in its outermost non-unit dimension
+    uint32_t ob[4] = {(uint32_t)SUB_W, p->m_box[0], p->m_box[1], p->m_box[2]};
+    const int hd = p->m_box[2] > 1 ? 2 : (p->m_box[1] > 1 ? 1 : 0);
+    ob[1 + hd] /= 2;
+    d.wg_off[hd] = ob[1 + hd];
+    uint64_t os[3];
+    row_strides(p->ldo, os);
+    if (encode_tmap_bf16_sw64(&em.out, p->out, 4, od, os, ob)) return 1;
+    const uint32_t rb[4] = {(uint32_t)SUB_W, p->m_box[0], p->m_box[1], p->m_box[2]};
+    if (p->res1 != nullptr) {
+      row_strides(p->ld1, os);
+      if (encode_tmap_bf16_sw64(&em.res1, p->res1, 4, od, os, rb)) return 1;
+    }
+    if (p->res2 != nullptr) {
+      row_strides(p->ld2, os);
+      if (encode_tmap_bf16_sw64(&em.res2, p->res2, 4, od, os, rb)) return 1;
+    }
+  }
+
   CUtensorMap tmA;
   if (encode_tmap_bf16(&tmA, p->a_ptr, 5, p->a_dims, p->a_strides, p->a_box)) return 1;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   switch (bn) {
-    case 32: return launch<32>(p, tmA, d, st);
-    case 64: return launch<64>(p, tmA, d, st);
-    case 128: return launch<128>(p, tmA, d, st);
-    case 160: return launch<160>(p, tmA, d, st);
-    case 256: return launch<256>(p, tmA, d, st);
+    case 32: return launch<32>(p, tmA, em, d, st);
+    case 64: return launch<64>(p, tmA, em, d, st);
+    case 128: return launch<128>(p, tmA, em, d, st);
+    case 160: return launch<160>(p, tmA, em, d, st);
+    case 256: return launch<256>(p, tmA, em, d, st);
     default: set_error("b200svd_gemm: unsupported N tile %d", bn); return 1;
   }
 }

@@ -99,6 +99,13 @@ __device__ __forceinline__ void tma_load_5d(void* smem, const CUtensorMap* m, ui
 }
 
 // TMA tiled store (shared -> global, bulk async group); out-of-bounds parts of the box are clipped by hardware
+__device__ __forceinline__ void tma_store_4d(const CUtensorMap* m, const void* smem, int c0, int c1, int c2, int c3) {
+  asm volatile(
+      "cp.async.bulk.tensor.4d.global.shared::cta.tile.bulk_group [%0, {%2, %3, %4, %5}], [%1];" ::"l"(
+          reinterpret_cast<uint64_t>(m)),
+      "r"(smem_u32(smem)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+      : "memory");
+}
 __device__ __forceinline__ void tma_store_5d(const CUtensorMap* m, const void* smem, int c0, int c1, int c2, int c3,
                                              int c4) {
   asm volatile(
