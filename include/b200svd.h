@@ -104,6 +104,23 @@ int b200svd_gemm_pair_mode(int mode);
 int b200svd_flash_attn(const void* qkv, int64_t ldqkv, void* out, int64_t ldo, int n, int s, int heads, float scale,
                        void* stream);
 
+/* ---- FlashAttention forward, head dim 80 (wgmma + TMA) -----------------------------------------------------
+ * Self-attention of the OpenCLIP ViT-H/14 image tower of the SVD conditioner (open_clip ResidualAttentionBlock,
+ * nn.MultiheadAttention with 16 heads of 80; encoders/modules.py:697-729).  Same contract as b200svd_flash_attn with
+ * head dim 80: qkv [(n s), ldqkv] bf16, columns [q | k | v] each heads*80 wide (the in_proj output), out [(n s), ldo]
+ * bf16.  qkv and out 16-byte aligned, leading dims multiples of 8, ldqkv >= 3*heads*80, ldo >= heads*80. */
+int b200svd_flash_attn_d80(const void* qkv, int64_t ldqkv, void* out, int64_t ldo, int n, int s, int heads,
+                           float scale, void* stream);
+
+/* ---- CLIP image preprocessing + patch gather (ViT-H/14) ------------------------------------------------------
+ * FrozenOpenCLIPImageEmbedder.preprocess (encoders/modules.py:624-636): kornia resize to 224x224 (antialias Gaussian
+ * blur with reflect borders, then bicubic align_corners=True), (x+1)/2, CLIP mean/std normalisation; written as the
+ * A operand of the 14x14/stride-14 patch GEMM.  x: [n][3][h][w] fp32 contiguous; out: bf16 [(n*256)][ldp], column
+ * (kh*14 + kw)*3 + c, columns 588..ldp-1 zero (ldp multiple of 8, >= 592).  taps_y / taps_x: HOST arrays of the
+ * normalised 1-D Gaussian taps (odd counts <= 63, reflect padding ky/2 < h, kx/2 < w); {1.0f} = no blur. */
+int b200svd_clip_preprocess(const float* x, int n, int h, int w, void* out, int64_t ldp, const float* taps_y, int ky,
+                            const float* taps_x, int kx, void* stream);
+
 /* Kept for ABI compatibility (no reference counterpart): records a softmax variant 3..5 and returns the previous one.
  * The sm_90 kernel has a single softmax organisation whatever the variant.  Other values only query. */
 int b200svd_flash_attn_variant(int v);

@@ -95,6 +95,8 @@ _P, _I64, _I, _F = C.c_void_p, C.c_int64, C.c_int, C.c_float
 PROTOTYPES = {
     "b200svd_gemm": [C.POINTER(GemmParams), _P],
     "b200svd_flash_attn": [_P, _I64, _P, _I64, _I, _I, _I, _F, _P],
+    "b200svd_flash_attn_d80": [_P, _I64, _P, _I64, _I, _I, _I, _F, _P],
+    "b200svd_clip_preprocess": [_P, _I, _I, _I, _P, _I64, _P, _I, _P, _I, _P],
     "b200svd_small_attn": [_P, _I64, _P, _I64, _P, _I64, _P, _I64, _I, _I, _I, _I, _I, _I, _F, _P],
     "b200svd_pixel_attn": [_P, _I64, _P, _I64, _P, _I64, _P, _I64, _I, _I, _I, _I, _I, _F, _P],
     "b200svd_gn_stats": [_P, _I64, _I64, _I64, _I, _P, _P, _P, _P],

@@ -568,3 +568,60 @@ def vae_encoder_param_shapes(cfg: VaeConfig) -> Dict[str, tuple]:
             _conv(d, "conv_out", cin, cout)
     _conv(d, "quant_conv", 2 * cfg.z_channels, 2 * cfg.z_channels, 1)
     return d
+
+
+# --------------------------------------------------------------------------------------------------------------
+# OpenCLIP ViT-H/14 image tower of the conditioner (FrozenOpenCLIPImageEmbedder, reference
+# code/models/svd/sgm/modules/encoders/modules.py:574-733 -> open_clip 2.24 VisionTransformer, visual tower only)
+# --------------------------------------------------------------------------------------------------------------
+@dataclass(frozen=True)
+class ClipVisionConfig:
+    """Defaults = open_clip's ViT-H-14 vision config (width 1280, 32 layers, head width 80, MLP ratio 4, embed 1024)."""
+    image_size: int = 224
+    patch_size: int = 14
+    width: int = 1280
+    layers: int = 32
+    heads: int = 16
+    mlp: int = 5120
+    output_dim: int = 1024
+    eps: float = 1e-5
+
+    @property
+    def head_dim(self) -> int:
+        return self.width // self.heads
+
+    @property
+    def grid(self) -> int:
+        return self.image_size // self.patch_size
+
+    @property
+    def tokens(self) -> int:
+        return self.grid * self.grid + 1
+
+
+CLIP_TINY = ClipVisionConfig(width=160, layers=2, heads=2, mlp=640)
+"""Reduced same-topology tower for fast parity tests: head dim stays 80, still 224 / 14 and a 1024-wide projection."""
+
+
+def clip_visual_param_shapes(cfg: ClipVisionConfig) -> Dict[str, tuple]:
+    """Name -> shape of open_clip's `model.visual.state_dict()` (VisionTransformer with the default options of
+    ViT-H-14: no conv bias, class token, learned positional embedding, ln_pre, pre-LN ResidualAttentionBlocks over
+    nn.MultiheadAttention (fused in_proj), ln_post, `proj` [width, output_dim]).  In the SVD checkpoint these keys sit
+    under `conditioner.embedders.0.open_clip.model.visual.`.  Restated from open_clip's published source: neither
+    open_clip nor a checkpoint is available offline, so this layout is not checked against one."""
+    w, p = cfg.width, cfg.patch_size
+    d: Dict[str, tuple] = {"conv1.weight": (w, 3, p, p), "class_embedding": (w,),
+                           "positional_embedding": (cfg.tokens, w)}
+    _norm(d, "ln_pre", w)
+    for i in range(cfg.layers):
+        b = f"transformer.resblocks.{i}"
+        _norm(d, b + ".ln_1", w)
+        d[b + ".attn.in_proj_weight"] = (3 * w, w)
+        d[b + ".attn.in_proj_bias"] = (3 * w,)
+        _lin(d, b + ".attn.out_proj", w, w)
+        _norm(d, b + ".ln_2", w)
+        _lin(d, b + ".mlp.c_fc", w, cfg.mlp)
+        _lin(d, b + ".mlp.c_proj", cfg.mlp, w)
+    _norm(d, "ln_post", w)
+    d["proj"] = (w, cfg.output_dim)
+    return d

@@ -94,6 +94,11 @@ int encode_tmap_bf16_sw64(CUtensorMap* out, const void* gptr, int rank, const ui
   return encode_impl(out, gptr, rank, dims, strides_bytes, box, CU_TENSOR_MAP_SWIZZLE_64B);
 }
 
+int encode_tmap_bf16_sw32(CUtensorMap* out, const void* gptr, int rank, const uint64_t* dims,
+                          const uint64_t* strides_bytes, const uint32_t* box) {
+  return encode_impl(out, gptr, rank, dims, strides_bytes, box, CU_TENSOR_MAP_SWIZZLE_32B);
+}
+
 int sm_count() {
   static int n[B200_MAX_DEVICES] = {};
   const int slot = dev_slot();

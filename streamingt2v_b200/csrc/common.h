@@ -21,6 +21,9 @@ int encode_tmap_bf16_noswz(CUtensorMap* out, const void* gptr, int rank, const u
 // same, 64-byte swizzle (inner box extent 32 bf16)
 int encode_tmap_bf16_sw64(CUtensorMap* out, const void* gptr, int rank, const uint64_t* dims,
                           const uint64_t* strides_bytes, const uint32_t* box);
+// same, 32-byte swizzle (inner box extent 16 bf16)
+int encode_tmap_bf16_sw32(CUtensorMap* out, const void* gptr, int rank, const uint64_t* dims,
+                          const uint64_t* strides_bytes, const uint32_t* box);
 
 int sm_count();
 

@@ -153,6 +153,25 @@ __device__ __forceinline__ uint64_t smem_desc_mn_sw128(uint32_t saddr) {
   d |= (uint64_t)1 << 62;
   return d;
 }
+// K-major operand, 32-byte swizzle: rows of 16 x 16-bit (= 32 B, one k16 step), 8-row groups 256 B apart (the tile a
+// SWIZZLE_32B TMA box with a 16-element inner extent writes).
+__device__ __forceinline__ uint64_t smem_desc_k_sw32(uint32_t saddr) {
+  uint64_t d = 0;
+  d |= (uint64_t)((saddr >> 4) & 0x3FFF);
+  d |= (uint64_t)1 << 16;           // LBO (unused for swizzled K-major) = 1
+  d |= (uint64_t)(256 >> 4) << 32;  // SBO = 256 B
+  d |= (uint64_t)3 << 62;           // layout type SWIZZLE_32B
+  return d;
+}
+// MN-major operand, 32-byte swizzle: smem tile is [K rows][16 MN elements = 32 B]; 8-row (K) groups 256 B apart.
+__device__ __forceinline__ uint64_t smem_desc_mn_sw32(uint32_t saddr) {
+  uint64_t d = 0;
+  d |= (uint64_t)((saddr >> 4) & 0x3FFF);
+  d |= (uint64_t)1 << 16;           // LBO: stride between 16-element MN atoms (single atom here)
+  d |= (uint64_t)(256 >> 4) << 32;  // SBO: stride between 8-deep K groups
+  d |= (uint64_t)3 << 62;
+  return d;
+}
 
 // ----------------------------------------------------------------------------------------------
 // small math helpers

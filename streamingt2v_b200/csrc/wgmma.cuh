@@ -24,6 +24,21 @@ template <int N>
 struct Wgmma;
 
 template <>
+struct Wgmma<16> {
+  static constexpr int R = 8;
+  __device__ __forceinline__ static void rs_tb(float (&d)[R], const uint32_t (&a)[4], uint64_t db,
+                                             uint32_t scale_d) {
+    asm volatile(
+        "{\n.reg .pred p;\n"
+        "setp.ne.b32 p, %13, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7}, {%8, %9, %10, %11}, %12, p, 1, 1, 1;\n"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(scale_d));
+  }
+};
+
+template <>
 struct Wgmma<32> {
   static constexpr int R = 16;
   __device__ __forceinline__ static void ss(float (&d)[R], uint64_t da, uint64_t db, uint32_t scale_d) {

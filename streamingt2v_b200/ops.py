@@ -338,7 +338,8 @@ def _conv_common(x, a_dims, a_strides, a_box, w, Cout, K, taps, m_ext, m_box, m_
 # ----------------------------------------------------------------------------------------------------------------
 # attention
 # ----------------------------------------------------------------------------------------------------------------
-_FAMILY = {"b200svd_flash_attn": "flash_attn", "b200svd_small_attn": "small_attn", "b200svd_pixel_attn": "pixel_attn", "b200svd_gn_stats": "groupnorm",
+_FAMILY = {"b200svd_flash_attn": "flash_attn", "b200svd_flash_attn_d80": "flash_attn",
+           "b200svd_clip_preprocess": "clip_preprocess", "b200svd_small_attn": "small_attn", "b200svd_pixel_attn": "pixel_attn", "b200svd_gn_stats": "groupnorm",
            "b200svd_gn_stats_partials": "groupnorm",
            "b200svd_gn_apply": "groupnorm", "b200svd_layernorm": "layernorm"}
 
@@ -363,6 +364,67 @@ def flash_attn(qkv, n, s, heads, out=None):
         out = torch.empty((n * s, Cc), dtype=torch.bfloat16, device=qkv.device)
     _call("b200svd_flash_attn", _ptr(qkv), qkv.stride(0), _ptr(out), out.stride(0), n, s, heads, 64 ** -0.5, _stream(),
           flops=4.0 * n * heads * float(s) * s * 64, nbytes=2.0 * n * s * 4 * Cc, desc=f"n{n} s{s} h{heads}")
+    return out
+
+
+def flash_attn_d80(qkv, n, s, heads, out=None):
+    """Head dim 80 (CLIP ViT-H/14 tower).  qkv: [(n s), >= 3*heads*80] bf16 (row stride free; columns [q | k | v]
+    each heads*80 wide) -> [(n s), heads*80]."""
+    assert qkv.dtype == torch.bfloat16 and qkv.dim() == 2 and qkv.stride(1) == 1
+    Cc = heads * 80
+    assert qkv.shape[0] == n * s and qkv.shape[1] >= 3 * Cc
+    if out is None:
+        out = torch.empty((n * s, Cc), dtype=torch.bfloat16, device=qkv.device)
+    assert out.dtype == torch.bfloat16 and out.stride(1) == 1 and out.shape == (n * s, Cc)
+    _call("b200svd_flash_attn_d80", _ptr(qkv), qkv.stride(0), _ptr(out), out.stride(0), n, s, heads, 80 ** -0.5,
+          _stream(), flops=4.0 * n * heads * float(s) * s * 80, nbytes=2.0 * n * s * 4 * Cc,
+          desc=f"d80 n{n} s{s} h{heads}")
+    return out
+
+
+CLIP_PATCH_K = 14 * 14 * 3          # 588 columns of the patch-embedding A operand
+CLIP_PATCH_LD = 592                 # padded to a multiple of 8 (16-byte TMA rows)
+
+
+def clip_preprocess(x, taps_y, taps_x, out=None):
+    """CLIP preprocessing + ViT-H/14 patch gather.  x: [n, 3, H, W] fp32 contiguous in [-1, 1]; taps_y / taps_x: the
+    normalised 1-D Gaussian antialias taps (host sequences, odd lengths; [1.0] = no blur).
+    Returns the patch GEMM's A operand, bf16 [(n 256), 592], column (kh*14 + kw)*3 + c, columns 588.. zero."""
+    assert x.dtype == torch.float32 and x.dim() == 4 and x.shape[1] == 3 and x.is_contiguous()
+    n, _, H, W = x.shape
+    if out is None:
+        out = torch.empty((n * 256, CLIP_PATCH_LD), dtype=torch.bfloat16, device=x.device)
+    assert out.dtype == torch.bfloat16 and out.stride(1) == 1 and out.shape[0] == n * 256
+    ty = (C.c_float * len(taps_y))(*[float(v) for v in taps_y])
+    tx = (C.c_float * len(taps_x))(*[float(v) for v in taps_x])
+    _call("b200svd_clip_preprocess", _ptr(x), n, H, W, _ptr(out), out.stride(0), ty, len(taps_y), tx, len(taps_x),
+          _stream(), nbytes=4.0 * x.numel() + 2.0 * out.numel(), desc=f"n{n} {H}x{W} taps{len(taps_y)}x{len(taps_x)}")
+    return out
+
+
+def linear_grouped(x, w, bias=None, *, groups, out, out_group_rows, **epi):
+    """`linear` over `groups` equal blocks of rows of x ([(groups rows), K]) whose outputs land in blocks of
+    out_group_rows rows of `out`: input row r of group g -> output row g * out_group_rows + r (the GEMM's out_rs).
+    Used to write the patch embedding straight into token rows 1..256 of each image."""
+    assert x.dtype == torch.bfloat16 and x.dim() == 2 and x.stride(1) == 1
+    M, K = x.shape
+    assert M % groups == 0
+    rows = M // groups
+    N = w.shape[-2]
+    assert w.shape[-1] == K and w.is_contiguous() and out.stride(-1) == 1
+    assert out.shape[1] == N and (groups - 1) * out_group_rows + rows <= out.shape[0]
+    ld = x.stride(0)
+    big = ld * 2 * max(M, 1)
+    act = epi.pop("act", ACT_NONE)
+    out_fp32 = epi.pop("out_fp32", False)
+    kw = _epi_kwargs(M, N, out, bias, epi.pop("fvec", None), epi.pop("rows_per_frame", 1), act,
+                     epi.pop("s_acc", 1.0), epi.pop("res1", None), epi.pop("s1", 1.0), epi.pop("res2", None),
+                     epi.pop("s2", 1.0), out_fp32)
+    assert not epi, f"unknown epilogue args {list(epi)}"
+    gemm_raw(a=x, a_dims=(K, rows, groups, 1, 1), a_strides=(ld * 2, rows * ld * 2, big, big),
+             a_box=(64, 128, 1, 1, 1), w=w, n=N, k=K, taps=1, tap_off=[(0, 0, 0, 0, 0)], m_ext=(rows, groups, 1),
+             m_box=(128, 1, 1), m_adim=(1, 2, 3), out=out, ldo=out.stride(0),
+             out_rs=(1, out_group_rows, groups * out_group_rows), **kw)
     return out
 
 

@@ -72,3 +72,29 @@ def pack_geglu(w: torch.Tensor, b: torch.Tensor, device):
 
 def f32(t: torch.Tensor, device) -> torch.Tensor:
     return t.detach().to(device=device, dtype=torch.float32).contiguous()
+
+
+# ---- OpenCLIP ViT-H/14 image tower (conditioner.py) -------------------------------------------------------------
+def pack_clip_patch(w: torch.Tensor, device) -> torch.Tensor:
+    """conv1 weight [width, 3, 14, 14] (no bias) -> [1, width, 592] in the column order of the preprocessing kernel's
+    patch rows: column (kh*14 + kw)*3 + c, zero-padded from 588 to 592."""
+    width, c, kh, kw = w.shape
+    return _bf16(pad_k(w.float().permute(0, 2, 3, 1).reshape(width, kh * kw * c))[None], device)
+
+
+def pack_clip_class_row(class_embedding: torch.Tensor, pos: torch.Tensor, device) -> torch.Tensor:
+    """Token 0 of every image before ln_pre: class_embedding + positional_embedding[0], one bf16 row [1, width]."""
+    return _bf16((class_embedding.float() + pos.float()[0])[None], device)
+
+
+def pack_clip_patch_pos(pos: torch.Tensor, device) -> torch.Tensor:
+    """positional_embedding [257, width] -> bf16 [257, width] rows [0, pos[1], ..., pos[256]]: added with add_rows to
+    every image's token rows — patch tokens get their embedding, the class row (already holding pos[0]) zero."""
+    p = pos.float().clone()
+    p[0] = 0.0
+    return _bf16(p, device)
+
+
+def pack_clip_proj(proj: torch.Tensor, device) -> torch.Tensor:
+    """`proj` [width, output_dim] (x @ proj) -> nn.Linear layout [1, output_dim, width]."""
+    return pack_linear(proj.float().t(), device)

@@ -9,11 +9,11 @@ Mirrors, method for method, the reference's `StreamingSVD` LightningModule
     _autoregressive_generation    :293-356   chunk loop: condition on the previous chunk, keep frames after the first
                                              `num_conditional_frames`, concatenate, convert to [0, 255]
 It is host logic: frame bookkeeping on whole tensors (slicing, concatenation, range conversion — the reference's
-`result_processor.convert_range`, utils/result_processor.py:4-14).  The conditioner (OpenCLIP image tower + SD-VAE
-encoder, encoders/modules.py) is a "next" row and out of scope here: it is injected as a callable
+`result_processor.convert_range`, utils/result_processor.py:4-14).  The conditioner is injected as a callable
 `conditioner(svd_input_frame, num_frames) -> (c, uc)` with `crossattn [1,L,1024]`, `concat [1,4,h,w]`,
 `vector [num_frames,768]`, exactly what `conditioner.get_unconditional_conditioning` returns at
-streaming_svd.py:181-188.  The heavy components raise without the CUDA library; nothing here falls back to a CPU
+streaming_svd.py:181-188; `conditioner.B200SVDConditioner` is that callable on the project's kernels (OpenCLIP ViT-H/14
+image tower with CLIP preprocessing, SD-VAE encoder, fps / motion / cond_aug embeddings).  The heavy components raise without the CUDA library; nothing here falls back to a CPU
 implementation."""
 from __future__ import annotations
 
@@ -116,7 +116,7 @@ class B200StreamingSVDStage:
         if self.shard_decode or getattr(self.sampler, "cfg_parallel", False):
             # every rank of a sharded step / decode must integrate the SAME latent: rank 0's noise wins (the ranks'
             # generators are not assumed to be seeded alike).  The conditioner's cond_aug noise (streaming_svd.py:174)
-            # is drawn inside the injected callable and must be made rank-invariant there.
+            # is drawn inside the injected callable; B200SVDConditioner broadcasts rank 0's the same way.
             randn = dist_utils.broadcast_from_rank0(randn)
         extra = dict(image_only_indicator=torch.zeros(2 * batch_size, T, device=self.device), num_video_frames=T,
                      batch_size=2 * batch_size, num_conditional_frames=self.num_conditional_frames,
