@@ -100,7 +100,9 @@ int b200svd_gemm_pair_mode(int mode);
 /* ---- FlashAttention forward, head dim 64 (wgmma + TMA) -----------------------------------------------------
  * Spatial self-attention core of BasicTransformerBlock.attn1 (attention.py:320-351 SDPA / :427-446 xformers).
  * qkv: [(n s), ldqkv] bf16, columns [q | k | v] each heads*64 wide (output of the fused QKV projection);
- * out: [(n s), ldo] bf16.  softmax(q k^T * scale) v per (frame, head). */
+ * out: [(n s), ldo] bf16.  softmax(q k^T * scale) v per (frame, head).  Returns an error, before any launch, unless
+ * n, s, heads >= 1 with n, heads <= 65535, qkv and out are 16-byte aligned, leading dims are multiples of 8,
+ * ldqkv >= 3*heads*64 and ldo >= heads*64. */
 int b200svd_flash_attn(const void* qkv, int64_t ldqkv, void* out, int64_t ldo, int n, int s, int heads, float scale,
                        void* stream);
 
@@ -108,7 +110,7 @@ int b200svd_flash_attn(const void* qkv, int64_t ldqkv, void* out, int64_t ldo, i
  * Self-attention of the OpenCLIP ViT-H/14 image tower of the SVD conditioner (open_clip ResidualAttentionBlock,
  * nn.MultiheadAttention with 16 heads of 80; encoders/modules.py:697-729).  Same contract as b200svd_flash_attn with
  * head dim 80: qkv [(n s), ldqkv] bf16, columns [q | k | v] each heads*80 wide (the in_proj output), out [(n s), ldo]
- * bf16.  qkv and out 16-byte aligned, leading dims multiples of 8, ldqkv >= 3*heads*80, ldo >= heads*80. */
+ * bf16, and the same argument checks with 80 in place of 64. */
 int b200svd_flash_attn_d80(const void* qkv, int64_t ldqkv, void* out, int64_t ldo, int n, int s, int heads,
                            float scale, void* stream);
 

@@ -355,31 +355,28 @@ def _call(name, *args, flops=0.0, nbytes=0.0, desc=""):
         _prof_end(e0, (fam, desc) if desc else fam, flops, nbytes)
 
 
-def flash_attn(qkv, n, s, heads, out=None):
-    """qkv: [(n s), 3*heads*64] bf16 (row stride free) -> [(n s), heads*64]."""
+def _flash_attn(entry, d, desc, qkv, n, s, heads, out):
     assert qkv.dtype == torch.bfloat16 and qkv.dim() == 2 and qkv.stride(1) == 1
-    Cc = heads * 64
-    assert qkv.shape == (n * s, 3 * Cc)
+    Cc = heads * d
+    assert qkv.shape[0] == n * s and qkv.shape[1] >= 3 * Cc
     if out is None:
         out = torch.empty((n * s, Cc), dtype=torch.bfloat16, device=qkv.device)
-    _call("b200svd_flash_attn", _ptr(qkv), qkv.stride(0), _ptr(out), out.stride(0), n, s, heads, 64 ** -0.5, _stream(),
-          flops=4.0 * n * heads * float(s) * s * 64, nbytes=2.0 * n * s * 4 * Cc, desc=f"n{n} s{s} h{heads}")
+    assert out.dtype == torch.bfloat16 and out.stride(1) == 1 and out.shape == (n * s, Cc)
+    _call(entry, _ptr(qkv), qkv.stride(0), _ptr(out), out.stride(0), n, s, heads, d ** -0.5, _stream(),
+          flops=4.0 * n * heads * float(s) * s * d, nbytes=2.0 * n * s * 4 * Cc, desc=desc)
     return out
+
+
+def flash_attn(qkv, n, s, heads, out=None):
+    """qkv: [(n s), >= 3*heads*64] bf16 (row stride free; columns [q | k | v] each heads*64 wide)
+    -> [(n s), heads*64]."""
+    return _flash_attn("b200svd_flash_attn", 64, f"n{n} s{s} h{heads}", qkv, n, s, heads, out)
 
 
 def flash_attn_d80(qkv, n, s, heads, out=None):
     """Head dim 80 (CLIP ViT-H/14 tower).  qkv: [(n s), >= 3*heads*80] bf16 (row stride free; columns [q | k | v]
     each heads*80 wide) -> [(n s), heads*80]."""
-    assert qkv.dtype == torch.bfloat16 and qkv.dim() == 2 and qkv.stride(1) == 1
-    Cc = heads * 80
-    assert qkv.shape[0] == n * s and qkv.shape[1] >= 3 * Cc
-    if out is None:
-        out = torch.empty((n * s, Cc), dtype=torch.bfloat16, device=qkv.device)
-    assert out.dtype == torch.bfloat16 and out.stride(1) == 1 and out.shape == (n * s, Cc)
-    _call("b200svd_flash_attn_d80", _ptr(qkv), qkv.stride(0), _ptr(out), out.stride(0), n, s, heads, 80 ** -0.5,
-          _stream(), flops=4.0 * n * heads * float(s) * s * 80, nbytes=2.0 * n * s * 4 * Cc,
-          desc=f"d80 n{n} s{s} h{heads}")
-    return out
+    return _flash_attn("b200svd_flash_attn_d80", 80, f"d80 n{n} s{s} h{heads}", qkv, n, s, heads, out)
 
 
 CLIP_PATCH_K = 14 * 14 * 3          # 588 columns of the patch-embedding A operand

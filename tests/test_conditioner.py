@@ -142,26 +142,34 @@ def _err(lib, rc, word):
     assert word in msg.lower(), msg
 
 
+def _flash_entry(lib, d):
+    return lib.b200svd_flash_attn if d == 64 else lib.b200svd_flash_attn_d80
+
+
+@pytest.mark.parametrize("d", [64, 80])
 @pytest.mark.parametrize("which", ["qkv", "out"])
-def test_flash_attn_d80_rejects_misaligned(lib, which):
+def test_flash_attn_d80_rejects_misaligned(lib, which, d):
     qkv, out = BASE, BASE + 0x100000
     if which == "qkv":
         qkv += 8
     else:
         out += 8
-    _err(lib, lib.b200svd_flash_attn_d80(qkv, 3 * 160, out, 160, 1, 257, 2, 80 ** -0.5, None), "align")
+    C2 = 2 * d  # two heads
+    _err(lib, _flash_entry(lib, d)(qkv, 3 * C2, out, C2, 1, 257, 2, d ** -0.5, None), "align")
 
 
+@pytest.mark.parametrize("d", [64, 80])
 @pytest.mark.parametrize("args,word", [
-    (dict(ldqkv=3 * 160 + 4), "multiples of 8"),
-    (dict(ldqkv=3 * 160 - 8), "ldqkv"),
-    (dict(ldo=152), "ldo"),
-    (dict(s=0), "need n, s, heads"),
+    (lambda C2: dict(ldqkv=3 * C2 + 4), "multiples of 8"),
+    (lambda C2: dict(ldqkv=3 * C2 - 8), "ldqkv"),
+    (lambda C2: dict(ldo=C2 - 8), "ldo"),
+    (lambda C2: dict(s=0), "need n, s, heads"),
 ], ids=["ld_not_8", "ldqkv_short", "ldo_short", "empty"])
-def test_flash_attn_d80_rejects_bad_sizes(lib, args, word):
-    a = dict(ldqkv=3 * 160, ldo=160, n=1, s=257, heads=2)
-    a.update(args)
-    rc = lib.b200svd_flash_attn_d80(BASE, a["ldqkv"], BASE + 0x100000, a["ldo"], a["n"], a["s"], a["heads"], 0.1, None)
+def test_flash_attn_d80_rejects_bad_sizes(lib, args, word, d):
+    C2 = 2 * d  # two heads
+    a = dict(ldqkv=3 * C2, ldo=C2, n=1, s=257, heads=2)
+    a.update(args(C2))
+    rc = _flash_entry(lib, d)(BASE, a["ldqkv"], BASE + 0x100000, a["ldo"], a["n"], a["s"], a["heads"], 0.1, None)
     _err(lib, rc, word)
 
 
