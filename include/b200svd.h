@@ -69,7 +69,8 @@ typedef struct {
   const float* fvec;       /* [frames][ldf] fp32 or NULL */
   int64_t ldf;
   uint32_t rows_per_frame; /* frame index = row / rows_per_frame */
-  int32_t act;             /* B200SVD_ACT_* ; GEGLU halves the output width (weights must be tile-interleaved) */
+  int32_t act;             /* B200SVD_ACT_* ; GEGLU halves the output width (weights interleaved per tile: bn 128 or
+                              256, 0 = 256, n divisible by it) */
   float s_acc;
   const void* res1; /* bf16 [rows][ld1] or NULL */
   int64_t ld1;
@@ -96,6 +97,16 @@ int b200svd_gemm(const b200svd_gemm_params* p, void* stream);
 /* Kept for ABI compatibility (no reference counterpart): records a CTA-pair tile mode 0..3 and returns the previous
  * one.  sm_90 has no CTA-pair MMA; every launch uses single-CTA tiles whatever the mode.  Other values only query. */
 int b200svd_gemm_pair_mode(int mode);
+
+/* Schedule of the consumer warpgroups (no reference counterpart); returns the previous mode, other values only query.
+ *   0  cooperative everywhere: both warpgroups work on the same 128 x bn tile, 64 rows each.
+ *   1  alternating wherever it exists: each warpgroup computes whole 128 x bn tiles, the CTA's tiles in turn, so one
+ *      warpgroup's epilogue runs under the other's MMAs.  bf16 outputs written by TMA stores without gn_part, N tile
+ *      at most 160: a 256-wide tile runs as 128-wide tiles, except GEGLU, whose tile is fixed by its weights.
+ *   2  (default) alternating for launches of at least 2 tiles per SM whose tiles are short (taps x K blocks x 2 x bn
+ *      below 20000 tensor-core clocks) and bn other than 160, cooperative otherwise.
+ * Both schedules give bitwise the same output. */
+int b200svd_gemm_schedule(int mode);
 
 /* ---- FlashAttention forward, head dim 64 (wgmma + TMA) -----------------------------------------------------
  * Spatial self-attention core of BasicTransformerBlock.attn1 (attention.py:320-351 SDPA / :427-446 xformers).

@@ -18,6 +18,11 @@
 //                   and applies the epilogue to its accumulator registers.  bf16 outputs are written 32 columns at a
 //                   time through a shared-memory staging buffer and a TMA store; fp32 outputs are stored directly.
 // A convolution tap is a shifted box of the same activation view, so taps and K blocks form one reduction loop.
+//
+// Two schedules share the producers and the epilogue arithmetic.  "Cooperative" (mtgemm_kernel) is the one above.
+// "Alternating" (mtgemm_alt_kernel) gives whole 128 x BN tiles to the consumer warpgroups in turn (warpgroup w takes
+// the CTA's tiles w, w + 2, ...), so the epilogue of one tile runs under the MMAs of the next; it is chosen for bf16
+// launches of many short-K tiles, where the epilogue is a large share of a tile (b200svd_gemm_schedule).
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <stdlib.h>
@@ -25,6 +30,7 @@
 
 #include "../../include/b200svd.h"
 #include "common.h"
+#include "mtgemm_ring.h"
 #include "ptx.cuh"
 #include "wgmma.cuh"
 
@@ -64,7 +70,52 @@ struct GemmDev {
   uint32_t stages;     // depth of the A/B stage ring
   uint32_t res_slots;  // depth of the residual ring (bf16 outputs with residuals, else 0)
   uint32_t wg_off[3];  // row-box origin of the second consumer warpgroup's 64 rows (bf16 output stores)
+#ifdef MTGEMM_PHASE_CLOCKS
+  long long* phase_buf;  // [CTA][role][PC_N] clock sums, see PhaseClock
+#endif
 };
+
+// Where a thread's clocks go.  Only the measuring build (-DMTGEMM_PHASE_CLOCKS, scripts/bench_gemm_shapes.py) reads
+// the clock: mark(i) adds the time since the previous mark to counter i.  In the product build every call is empty.
+enum {
+  PC_RING_WAIT = 0,   // producer: waiting for a free stage; consumer: waiting for a full one
+  PC_MMA = 1,         // consumer: first wgmma of a stage to the wait that retires it
+  PC_RES_WAIT = 2,    // epilogue: waiting for a residual slot
+  PC_STORE_WAIT = 3,  // epilogue: until the previous TMA store has read its staging buffer, plus the named barrier
+  PC_EPI = 4,         // epilogue: everything else
+  PC_OTHER = 5,       // issue work of the producer, stepping over the other warpgroup's tiles
+  PC_TOTAL = 7,       // lifetime of the thread
+  PC_N = 8
+};
+#ifdef MTGEMM_PHASE_CLOCKS
+struct PhaseClock {
+  long long t0, last, acc[PC_N];
+  __device__ __forceinline__ PhaseClock() {
+    t0 = last = clock64();
+#pragma unroll
+    for (int i = 0; i < PC_N; ++i) acc[i] = 0;
+  }
+  __device__ __forceinline__ void mark(int i) {
+    const long long n = clock64();
+    acc[i] += n - last;
+    last = n;
+  }
+  // role: 0 = A/B producer, 1 and 2 = leader of the consumer warpgroups
+  __device__ __forceinline__ void write(long long* buf, int role) {
+    if (buf == nullptr) return;
+    acc[PC_TOTAL] = clock64() - t0;
+#pragma unroll
+    for (int i = 0; i < PC_N; ++i) buf[((size_t)blockIdx.x * 3 + role) * PC_N + i] += acc[i];
+  }
+};
+#define PC_BUF(p) ((p).phase_buf)
+#else
+struct PhaseClock {
+  __device__ __forceinline__ void mark(int) {}
+  __device__ __forceinline__ void write(long long*, int) {}
+};
+#define PC_BUF(p) nullptr
+#endif
 
 constexpr int BM = 128;
 constexpr int BK = 64;
@@ -83,7 +134,7 @@ constexpr int MAX_RES_SLOTS = 16;
 constexpr int GN_BYTES = 2 * 2 * 2 * SUB_W * 8;  // [warpgroup][buffer][quadrant][column][sum, sum of squares]
 constexpr int BAR_BYTES = 512;
 constexpr int FIXED_BYTES = STG_BYTES + GN_BYTES + BAR_BYTES;
-static_assert(2 * (MAX_STAGES + MAX_RES_SLOTS) * 8 <= BAR_BYTES, "barrier area");
+static_assert(2 * (MAX_STAGES + MAX_RES_SLOTS) * 8 + 16 <= BAR_BYTES, "barrier area and the tile counters");
 
 // Shared memory (offsets in bytes, every region 1024-byte aligned):
 //   [0, stages * STAGE_BYTES)   A/B stage ring
@@ -97,6 +148,7 @@ template <int BN>
 struct TileCfg {
   static constexpr int B_STAGE_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
+  static constexpr int FIXED = FIXED_BYTES;
   static constexpr int STAGES_FIT = (SMEM_LIMIT - FIXED_BYTES) / STAGE_BYTES;
   static constexpr int STAGES = STAGES_FIT > MAX_STAGES ? MAX_STAGES : STAGES_FIT;
   static constexpr int SUBTILES = BN / SUB_W;
@@ -108,6 +160,31 @@ struct TileCfg {
   static_assert(STAGES >= 4, "pipeline depth without residuals");
   static_assert(RES_SLOTS_AT_MIN >= 2, "two residuals need two ring slots");
   static_assert(STAGES * STAGE_BYTES + FIXED_BYTES <= SMEM_LIMIT, "shared memory budget");
+  static_assert(STAGE_BYTES % 1024 == 0, "stage alignment");
+  static_assert(BN % SUB_W == 0, "sub-tiles");
+};
+
+// Alternating schedule: a consumer warpgroup holds the whole 128 x BN accumulator (BN registers per thread, so
+// BN <= 160) and stages 128-row sub-tiles (8 KB, two buffers per warpgroup); no GroupNorm partials.
+constexpr int ALT_STG_SLOT_BYTES = BM * SUB_W * 2;
+constexpr int ALT_STG_BYTES = 2 * STG_SLOTS * ALT_STG_SLOT_BYTES;
+template <int BN>
+struct AltCfg {
+  static constexpr int B_STAGE_BYTES = BN * BK * 2;
+  static constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
+  static constexpr int FIXED = ALT_STG_BYTES + BAR_BYTES;
+  static constexpr int STAGES_FIT = (SMEM_LIMIT - FIXED) / STAGE_BYTES;
+  static constexpr int STAGES = STAGES_FIT > MAX_STAGES ? MAX_STAGES : STAGES_FIT;
+  static constexpr int SUBTILES = BN / SUB_W;
+  static constexpr int CONSUMER_REGS = 232;
+  static constexpr int PRODUCER_REGS = 40;
+  static constexpr int RES_SLOTS_AT_MIN = (SMEM_LIMIT - FIXED - MIN_STAGES * STAGE_BYTES) / RES_SLOT_BYTES;
+  static int res_slots_fit(int stages) { return (SMEM_LIMIT - FIXED - stages * STAGE_BYTES) / RES_SLOT_BYTES; }
+  static_assert(BN <= 160, "128 x BN accumulator in one warpgroup's registers");
+  static_assert(2 * 128 * CONSUMER_REGS + 128 * PRODUCER_REGS <= 65536, "register file");
+  static_assert(STAGES >= 4, "pipeline depth without residuals");
+  static_assert(RES_SLOTS_AT_MIN >= 2, "two residuals need two ring slots");
+  static_assert(STAGES * STAGE_BYTES + FIXED <= SMEM_LIMIT, "shared memory budget");
   static_assert(STAGE_BYTES % 1024 == 0, "stage alignment");
   static_assert(BN % SUB_W == 0, "sub-tiles");
 };
@@ -160,6 +237,76 @@ __device__ __forceinline__ uint32_t sw64_off(uint32_t row, uint32_t ch, uint32_t
   return row * 64u + ((ch ^ ((row >> 1) & 3u)) << 4) + cp * 4u;
 }
 
+// TMA producer of the A/B stage ring (one thread): the CTA's tiles in order, taps and K blocks of each.  Both
+// schedules run it unchanged; the ring is what orders the consumers.
+template <int BN>
+__device__ __forceinline__ void produce_ab(const GemmDev& p, const CUtensorMap* tmA, const CUtensorMap* tmB,
+                                           uint8_t* smem, uint64_t* full_bar, uint64_t* empty_bar) {
+  constexpr int STAGE_BYTES = A_STAGE_BYTES + BN * BK * 2;
+  PhaseClock pc;
+  uint32_t st = 0, ph = 0;
+  for (uint32_t tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+    uint32_t n_tile, mb1, mb2, mb3;
+    decode_tile(p, tile, n_tile, mb1, mb2, mb3);
+    int base[5] = {0, 0, 0, 0, 0};
+    base[p.m_adim[0]] += (int)mb1;
+    base[p.m_adim[1]] += (int)mb2;
+    base[p.m_adim[2]] += (int)mb3;
+    const int n0 = (int)(n_tile * BN);
+    for (uint32_t tap = 0; tap < p.taps; ++tap) {
+      const int c0 = p.tap_off[tap][0];
+      const int c1 = base[1] + p.tap_off[tap][1];
+      const int c2 = base[2] + p.tap_off[tap][2];
+      const int c3 = base[3] + p.tap_off[tap][3];
+      const int c4 = base[4] + p.tap_off[tap][4];
+#pragma unroll 1
+      for (uint32_t kb = 0; kb < p.kblocks; ++kb) {
+        pc.mark(PC_OTHER);
+        mbar_wait_parked(&empty_bar[st], ph ^ 1);
+        pc.mark(PC_RING_WAIT);
+        uint8_t* sa = smem + st * STAGE_BYTES;
+        mbar_expect_tx(&full_bar[st], STAGE_BYTES);
+        tma_load_5d(sa, tmA, &full_bar[st], c0 + (int)(kb * BK), c1, c2, c3, c4);
+        tma_load_3d(sa + A_STAGE_BYTES, tmB, &full_bar[st], (int)(kb * BK), n0, (int)tap);
+        if (++st == p.stages) {
+          st = 0;
+          ph ^= 1;
+        }
+      }
+    }
+  }
+  pc.write(PC_BUF(p), 0);
+}
+
+// TMA producer of the residual ring (one thread; bf16 outputs): sub-tile by sub-tile, res1 then res2, 128 rows x 32
+// columns a slot.  It runs ahead of the consumers by the depth of the ring, so a tile's residuals stream in during
+// its MMAs.
+__device__ __forceinline__ void produce_residuals(const GemmDev& p, const CUtensorMap* tmR1, const CUtensorMap* tmR2,
+                                                  uint8_t* res_smem, uint64_t* res_full, uint64_t* res_empty,
+                                                  uint32_t tile_out_w, uint32_t n_out) {
+  if (p.res1 != nullptr) prefetch_tmap(tmR1);
+  if (p.res2 != nullptr) prefetch_tmap(tmR2);
+  uint32_t slot = 0, ph = 0;
+  for (uint32_t tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+    uint32_t n_tile, mb1, mb2, mb3;
+    decode_tile(p, tile, n_tile, mb1, mb2, mb3);
+    const uint32_t otile0 = n_tile * tile_out_w;
+    for (uint32_t c = 0; c < tile_out_w / SUB_W && otile0 + c * SUB_W < n_out; ++c) {
+      for (int r = 0; r < 2; ++r) {
+        if ((r == 0 ? p.res1 : p.res2) == nullptr) continue;
+        mbar_wait_parked(&res_empty[slot], ph ^ 1);
+        mbar_expect_tx(&res_full[slot], RES_SLOT_BYTES);
+        tma_load_4d(res_smem + slot * RES_SLOT_BYTES, r == 0 ? tmR1 : tmR2, &res_full[slot],
+                    (int)(otile0 + c * SUB_W), (int)mb1, (int)mb2, (int)mb3);
+        if (++slot == p.res_slots) {
+          slot = 0;
+          ph ^= 1;
+        }
+      }
+    }
+  }
+}
+
 template <int BN>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 mtgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
@@ -205,60 +352,9 @@ mtgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
   if (wg == 0) {
     asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(Cfg::PRODUCER_REGS));
     if (threadIdx.x == 0) {
-      // ===================== TMA producer (A, B) =====================
-      uint32_t st = 0, ph = 0;
-      for (uint32_t tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-        uint32_t n_tile, mb1, mb2, mb3;
-        decode_tile(p, tile, n_tile, mb1, mb2, mb3);
-        int base[5] = {0, 0, 0, 0, 0};
-        base[p.m_adim[0]] += (int)mb1;
-        base[p.m_adim[1]] += (int)mb2;
-        base[p.m_adim[2]] += (int)mb3;
-        const int n0 = (int)(n_tile * BN);
-        for (uint32_t tap = 0; tap < p.taps; ++tap) {
-          const int c0 = p.tap_off[tap][0];
-          const int c1 = base[1] + p.tap_off[tap][1];
-          const int c2 = base[2] + p.tap_off[tap][2];
-          const int c3 = base[3] + p.tap_off[tap][3];
-          const int c4 = base[4] + p.tap_off[tap][4];
-#pragma unroll 1
-          for (uint32_t kb = 0; kb < p.kblocks; ++kb) {
-            mbar_wait_parked(&empty_bar[st], ph ^ 1);
-            uint8_t* sa = smem + st * Cfg::STAGE_BYTES;
-            mbar_expect_tx(&full_bar[st], Cfg::STAGE_BYTES);
-            tma_load_5d(sa, &tmA, &full_bar[st], c0 + (int)(kb * BK), c1, c2, c3, c4);
-            tma_load_3d(sa + A_STAGE_BYTES, &tmB, &full_bar[st], (int)(kb * BK), n0, (int)tap);
-            if (++st == stages) {
-              st = 0;
-              ph ^= 1;
-            }
-          }
-        }
-      }
+      produce_ab<BN>(p, &tmA, &tmB, smem, full_bar, empty_bar);
     } else if (threadIdx.x == 32 && rslots != 0) {
-      // ============ TMA producer (residuals of bf16 outputs): sub-tile by sub-tile, res1 then res2 ============
-      // It runs ahead of the consumers by the depth of the ring, so a tile's residuals stream in during its MMAs.
-      if (p.res1 != nullptr) prefetch_tmap(&tmR1);
-      if (p.res2 != nullptr) prefetch_tmap(&tmR2);
-      uint32_t slot = 0, ph = 0;
-      for (uint32_t tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-        uint32_t n_tile, mb1, mb2, mb3;
-        decode_tile(p, tile, n_tile, mb1, mb2, mb3);
-        const uint32_t otile0 = n_tile * tile_out_w;
-        for (uint32_t c = 0; c < tile_out_w / SUB_W && otile0 + c * SUB_W < n_out; ++c) {
-          for (int r = 0; r < 2; ++r) {
-            if ((r == 0 ? p.res1 : p.res2) == nullptr) continue;
-            mbar_wait_parked(&res_empty[slot], ph ^ 1);
-            mbar_expect_tx(&res_full[slot], RES_SLOT_BYTES);
-            tma_load_4d(res_smem + slot * RES_SLOT_BYTES, r == 0 ? &tmR1 : &tmR2, &res_full[slot],
-                        (int)(otile0 + c * SUB_W), (int)mb1, (int)mb2, (int)mb3);
-            if (++slot == rslots) {
-              slot = 0;
-              ph ^= 1;
-            }
-          }
-        }
-      }
+      produce_residuals(p, &tmR1, &tmR2, res_smem, res_full, res_empty, tile_out_w, n_out);
     }
     return;
   }
@@ -277,13 +373,16 @@ mtgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
   uint32_t rslot = 0, rph = 0;      // residual ring position
   uint32_t stg_it = 0;              // sub-tiles staged by this warpgroup so far
   float acc[R];
+  PhaseClock pc;
 
   for (uint32_t tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+    pc.mark(PC_EPI);
 #pragma unroll
     for (int i = 0; i < R; ++i) acc[i] = 0.f;
     uint32_t prev = 0;
     for (uint32_t i = 0; i < iters_per_tile; ++i) {
       mbar_wait(&full_bar[st], sph);
+      pc.mark(PC_RING_WAIT);
       const uint32_t sa = smem_u32(smem + st * Cfg::STAGE_BYTES);
       const uint64_t adesc = smem_desc_k_sw128(sa + cw * (A_STAGE_BYTES / 2));
       const uint64_t bdesc = smem_desc_k_sw128(sa + A_STAGE_BYTES);
@@ -296,6 +395,7 @@ mtgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
       wgmma_fence_regs(acc);
       // the MMAs of the previous stage have completed: hand it back to the producer
       wgmma_wait<1>();
+      pc.mark(PC_MMA);
       if (i > 0 && leader) mbar_arrive(&empty_bar[prev]);
       prev = st;
       if (++st == stages) {
@@ -304,6 +404,7 @@ mtgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
       }
     }
     wgmma_wait<0>();
+    pc.mark(PC_MMA);
     wgmma_fence_regs(acc);
     if (leader) mbar_arrive(&empty_bar[prev]);
 
@@ -340,6 +441,7 @@ mtgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
         const uint8_t* r1s = nullptr;
         const uint8_t* r2s = nullptr;
         uint32_t r1slot = 0, r2slot = 0;
+        pc.mark(PC_EPI);
         if (p.res1 != nullptr) {
           r1slot = rslot;
           mbar_wait(&res_full[rslot], rph);
@@ -358,6 +460,7 @@ mtgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
             rph ^= 1;
           }
         }
+        pc.mark(PC_RES_WAIT);
 #pragma unroll
         for (int jj = 0; jj < 4; ++jj) {
           const int j = 4 * c + jj;
@@ -440,8 +543,10 @@ mtgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
         }
         fence_proxy_async_smem();  // the staged values are read by the TMA store (async proxy)
         // the store issued one sub-tile ago has read the other staging buffer: it may be refilled next sub-tile
+        pc.mark(PC_EPI);
         if (leader) tma_store_wait_read0();
         named_bar_sync(5 + cw, 128);
+        pc.mark(PC_STORE_WAIT);
         if (leader) {
           if (r1s != nullptr) mbar_arrive(&res_empty[r1slot]);
           if (r2s != nullptr) mbar_arrive(&res_empty[r2slot]);
@@ -535,7 +640,265 @@ mtgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
       }
     }
   }
+  pc.mark(PC_EPI);
+  if (leader) pc.write(PC_BUF(p), 1 + cw);
   if (p.staged && leader) tma_store_wait_all();  // shared memory must outlive the last stores' reads
+}
+
+// The alternating schedule.  Producers, tile order and ring contents are those of mtgemm_kernel; what changes is who
+// consumes a tile.  Warpgroup w computes the CTA's tiles w, w + 2, ... whole (two m64nBNk16 per k16 step, rows 0-63
+// and 64-127 of the A stage against the same B descriptor) and is the only one to release their stages and residual
+// slots, so every "empty" barrier counts one arrival.  It steps over the other warpgroup's tiles by ring arithmetic
+// alone (mtgemm_ring.h).  Because the ring is filled in tile order, a warpgroup's next tile becomes full as the other
+// one nears the end of its MMAs: one warpgroup's epilogue runs under the other's MMAs.
+// An mbarrier wait sees one bit of phase, so a wait for fill j of a buffer also passes while fill j - 1 of that buffer
+// has not landed (the barrier is two phases behind: the same parity).  A warpgroup that only did arithmetic over the
+// other's tile could be that far ahead.  Two monotonic tile counters per warpgroup in shared memory rule it out: a
+// warpgroup starts the MMAs (the residual waits) of its tile t only when the other one has passed every stage wait
+// (residual wait) of tile t - 1, so every earlier fill of every buffer has landed.  The tensor cores are shared, so
+// waiting for the other warpgroup's MMAs costs nothing that was not already spent.
+// Per output element the k order, the wgmma k16 steps and the epilogue arithmetic are those of
+// mtgemm_kernel, so the results are bitwise the same.  bf16 staged outputs only, no GroupNorm partials.
+template <int BN>
+__global__ void __launch_bounds__(NUM_THREADS, 1)
+mtgemm_alt_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                  const __grid_constant__ CUtensorMap tmO, const __grid_constant__ CUtensorMap tmR1,
+                  const __grid_constant__ CUtensorMap tmR2, const GemmDev p) {
+  using Cfg = AltCfg<BN>;
+  constexpr int R = BN / 2;  // accumulator registers per thread and 64-row half
+  extern __shared__ __align__(1024) uint8_t smem[];
+  if ((smem_u32(smem) & 1023u) != 0) __trap();
+  const uint32_t stages = p.stages, rslots = p.res_slots;
+  uint8_t* res_smem = smem + stages * Cfg::STAGE_BYTES;
+  uint8_t* stg_smem = res_smem + rslots * RES_SLOT_BYTES;
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(stg_smem + ALT_STG_BYTES);
+  uint64_t* empty_bar = full_bar + MAX_STAGES;
+  uint64_t* res_full = empty_bar + MAX_STAGES;
+  uint64_t* res_empty = res_full + MAX_RES_SLOTS;
+  // tiles of the CTA's sequence whose stage waits / residual waits warpgroup w has passed: [w], [2 + w]
+  uint32_t* tiles_done = reinterpret_cast<uint32_t*>(res_empty + MAX_RES_SLOTS);
+
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  const int wg = warp >> 2;
+  const uint32_t iters_per_tile = p.taps * p.kblocks;
+  const bool geglu = (p.act == B200SVD_ACT_GEGLU);
+  const uint32_t n_out = geglu ? p.n / 2 : p.n;
+  const uint32_t tile_out_w = geglu ? (uint32_t)BN / 2 : (uint32_t)BN;
+
+  if (threadIdx.x == 0) {
+    prefetch_tmap(&tmA);
+    prefetch_tmap(&tmB);
+    prefetch_tmap(&tmO);
+    for (int i = 0; i < 4; ++i) tiles_done[i] = 0;
+    for (uint32_t s = 0; s < stages; ++s) {
+      mbar_init(&full_bar[s], 1);
+      mbar_init(&empty_bar[s], 1);  // released by the warpgroup that owns the tile
+    }
+    for (uint32_t s = 0; s < rslots; ++s) {
+      mbar_init(&res_full[s], 1);
+      mbar_init(&res_empty[s], 1);
+    }
+    fence_barrier_init();
+  }
+  __syncthreads();
+
+  if (wg == 0) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(Cfg::PRODUCER_REGS));
+    if (threadIdx.x == 0) {
+      produce_ab<BN>(p, &tmA, &tmB, smem, full_bar, empty_bar);
+    } else if (threadIdx.x == 32 && rslots != 0) {
+      produce_residuals(p, &tmR1, &tmR2, res_smem, res_full, res_empty, tile_out_w, n_out);
+    }
+    return;
+  }
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(Cfg::CONSUMER_REGS));
+
+  // ===================== consumer warpgroups =====================
+  const uint32_t cw = (uint32_t)(wg - 1);
+  const int wl = warp & 3;  // warp of the warpgroup: rows 16 wl .. 16 wl + 15 of both 64-row halves
+  const int rq = lane >> 2, cq = lane & 3;
+  const bool leader = (threadIdx.x & 127) == 0;
+  const uint32_t lb1 = p.m_lb[0], lb2 = p.m_lb[1];
+  const uint32_t nres = (p.res1 != nullptr ? 1u : 0u) + (p.res2 != nullptr ? 1u : 0u);
+  RingPos ab = {0, 0};   // A/B ring position
+  RingPos rr = {0, 0};   // residual ring position
+  uint32_t stg_it = 0;   // sub-tiles staged by this warpgroup so far
+  float acc0[R], acc1[R];  // rows 0-63 and 64-127 of the tile
+  PhaseClock pc;
+
+  uint32_t t = 0;  // index of the tile in this CTA's sequence
+  for (uint32_t tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x, ++t) {
+    pc.mark(PC_EPI);
+    if (alt_owner(t) != cw) {
+      // The other warpgroup's tile: step over its stages and residual slots.  If none of this warpgroup's follows,
+      // it is done.
+      if (tile + gridDim.x >= p.total_tiles) break;
+      ring_advance(ab, iters_per_tile, stages);
+      if (rslots != 0) ring_advance(rr, tile_res_slots(tile % p.n_tiles, tile_out_w, n_out, SUB_W, nres), rslots);
+      continue;
+    }
+    while (ld_acquire_shared(&tiles_done[1 - cw]) < t) {  // the other warpgroup has seen tile t - 1's stages land
+    }
+    pc.mark(PC_OTHER);
+#pragma unroll
+    for (int i = 0; i < R; ++i) acc0[i] = acc1[i] = 0.f;
+    uint32_t prev = 0;
+    for (uint32_t i = 0; i < iters_per_tile; ++i) {
+      mbar_wait(&full_bar[ab.idx], ab.phase);
+      pc.mark(PC_RING_WAIT);
+      // the tile's last stage has landed: the other warpgroup may queue its MMAs behind these
+      if (leader && i + 1 == iters_per_tile) st_release_shared(&tiles_done[cw], t + 1);
+      const uint32_t sa = smem_u32(smem + ab.idx * Cfg::STAGE_BYTES);
+      const uint64_t adesc0 = smem_desc_k_sw128(sa);
+      const uint64_t adesc1 = smem_desc_k_sw128(sa + A_STAGE_BYTES / 2);
+      const uint64_t bdesc = smem_desc_k_sw128(sa + A_STAGE_BYTES);
+      wgmma_fence_regs(acc0);
+      wgmma_fence_regs(acc1);
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < BK / 16; ++kk) {  // +16 elements along K = +32 B inside the swizzle atom
+        Wgmma<BN>::ss(acc0, adesc0 + (uint64_t)(kk * 2), bdesc + (uint64_t)(kk * 2), 1u);
+        Wgmma<BN>::ss(acc1, adesc1 + (uint64_t)(kk * 2), bdesc + (uint64_t)(kk * 2), 1u);
+      }
+      wgmma_commit();
+      wgmma_fence_regs(acc0);
+      wgmma_fence_regs(acc1);
+      // the MMAs of the previous stage have completed: hand it back to the producer
+      wgmma_wait<1>();
+      pc.mark(PC_MMA);
+      if (i > 0 && leader) mbar_arrive(&empty_bar[prev]);
+      prev = ab.idx;
+      ring_step(ab, stages);
+    }
+    wgmma_wait<0>();
+    pc.mark(PC_MMA);
+    wgmma_fence_regs(acc0);
+    wgmma_fence_regs(acc1);
+    if (leader) mbar_arrive(&empty_bar[prev]);
+
+    // ----- epilogue: thread holds rows 64 hh + 16 wl + rq + 8 h, columns 8 j + 2 cq + {0, 1} (accHH[4 j + 2 h + e])
+    uint32_t n_tile, mb1, mb2, mb3;
+    decode_tile(p, tile, n_tile, mb1, mb2, mb3);
+    const uint32_t n0 = n_tile * BN;
+    const uint32_t otile0 = n_tile * tile_out_w;
+    const float* fv[2][2];
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const uint32_t r = (uint32_t)(64 * hh + 16 * wl + rq + 8 * h);
+        const uint32_t m1 = mb1 + (r & ((1u << lb1) - 1));
+        const uint32_t m2 = mb2 + ((r >> lb1) & ((1u << lb2) - 1));
+        const uint32_t m3 = mb3 + (r >> (lb1 + lb2));
+        const bool valid = (m1 < p.m_ext[0]) && (m2 < p.m_ext[1]) && (m3 < p.m_ext[2]);
+        const int64_t row = (int64_t)m1 * p.out_rs[0] + (int64_t)m2 * p.out_rs[1] + (int64_t)m3 * p.out_rs[2];
+        fv[hh][h] = (p.fvec != nullptr && valid) ? p.fvec + (int64_t)((uint32_t)row / p.rows_per_frame) * p.ldf
+                                                 : nullptr;
+      }
+    }
+    constexpr int NJ = BN / 8;
+    if (rslots != 0) {
+      pc.mark(PC_EPI);
+      while (ld_acquire_shared(&tiles_done[2 + 1 - cw]) < t) {  // ... and tile t - 1's residual slots
+      }
+      pc.mark(PC_RES_WAIT);
+    }
+#pragma unroll
+    for (int c = 0; c < Cfg::SUBTILES; ++c) {
+      if (geglu && c >= Cfg::SUBTILES / 2) break;  // gate columns are consumed with their value columns
+      if (otile0 + (uint32_t)(c * SUB_W) >= n_out) break;
+      uint8_t* stg = stg_smem + (cw * STG_SLOTS + (stg_it & 1)) * ALT_STG_SLOT_BYTES;
+      // residual sub-tiles (all 128 rows), in the order the residual producer loads them
+      const uint8_t* r1s = nullptr;
+      const uint8_t* r2s = nullptr;
+      uint32_t r1slot = 0, r2slot = 0;
+      pc.mark(PC_EPI);
+      if (p.res1 != nullptr) {
+        r1slot = rr.idx;
+        mbar_wait(&res_full[rr.idx], rr.phase);
+        r1s = res_smem + rr.idx * RES_SLOT_BYTES;
+        ring_step(rr, rslots);
+      }
+      if (p.res2 != nullptr) {
+        r2slot = rr.idx;
+        mbar_wait(&res_full[rr.idx], rr.phase);
+        r2s = res_smem + rr.idx * RES_SLOT_BYTES;
+        ring_step(rr, rslots);
+      }
+      pc.mark(PC_RES_WAIT);
+#pragma unroll
+      for (int jj = 0; jj < 4; ++jj) {
+        const int j = 4 * c + jj;
+        const uint32_t tcol = (uint32_t)(8 * j + 2 * cq);
+        const uint32_t ocol = otile0 + tcol;
+        const bool in0 = ocol < n_out, in1 = ocol + 1 < n_out;
+        float bv[2], gbv[2];
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const bool in = e == 0 ? in0 : in1;
+          bv[e] = (p.bias != nullptr && in) ? __ldg(p.bias + n0 + tcol + e) : 0.f;
+          gbv[e] = (geglu && p.bias != nullptr) ? __ldg(p.bias + n0 + BN / 2 + tcol + e) : 0.f;
+        }
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh) {
+          float(&acc)[R] = hh == 0 ? acc0 : acc1;
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const uint32_t off = sw64_off((uint32_t)(64 * hh + 16 * wl + rq + 8 * h), (uint32_t)jj, (uint32_t)cq);
+            float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+            float g0 = 0.f, g1 = 0.f;
+            if (p.bias != nullptr) {
+              v0 += bv[0];
+              v1 += bv[1];
+            }
+            if (fv[hh][h] != nullptr) {
+              v0 += in0 ? __ldg(fv[hh][h] + ocol) : 0.f;
+              v1 += in1 ? __ldg(fv[hh][h] + ocol + 1) : 0.f;
+            }
+            if (geglu) {
+              g0 = acc[4 * (j + NJ / 2) + 2 * h];
+              g1 = acc[4 * (j + NJ / 2) + 2 * h + 1];
+              if (p.bias != nullptr) {
+                g0 += gbv[0];
+                g1 += gbv[1];
+              }
+            }
+            v0 = epi_act(p, geglu, v0, g0);
+            v1 = epi_act(p, geglu, v1, g1);
+            if (r1s != nullptr) {
+              const uint32_t w = *reinterpret_cast<const uint32_t*>(r1s + off);
+              v0 = __fmaf_rn(p.s1, bf16_lo(w), v0);
+              v1 = __fmaf_rn(p.s1, bf16_hi(w), v1);
+            }
+            if (r2s != nullptr) {
+              const uint32_t w = *reinterpret_cast<const uint32_t*>(r2s + off);
+              v0 = __fmaf_rn(p.s2, bf16_lo(w), v0);
+              v1 = __fmaf_rn(p.s2, bf16_hi(w), v1);
+            }
+            *reinterpret_cast<uint32_t*>(stg + off) = pack_bf16x2(v0, v1);
+          }
+        }
+      }
+      fence_proxy_async_smem();  // the staged values are read by the TMA store (async proxy)
+      pc.mark(PC_EPI);
+      // the store issued one sub-tile ago has read the other staging buffer: it may be refilled next sub-tile
+      if (leader) tma_store_wait_read0();
+      named_bar_sync(5 + (int)cw, 128);
+      pc.mark(PC_STORE_WAIT);
+      if (leader) {
+        if (r1s != nullptr) mbar_arrive(&res_empty[r1slot]);
+        if (r2s != nullptr) mbar_arrive(&res_empty[r2slot]);
+        tma_store_4d(&tmO, stg, (int)(otile0 + c * SUB_W), (int)mb1, (int)mb2, (int)mb3);  // the tile's row box
+        tma_store_commit();
+      }
+      ++stg_it;
+    }
+    if (leader && rslots != 0) st_release_shared(&tiles_done[2 + cw], t + 1);
+  }
+  pc.mark(PC_EPI);
+  if (leader) pc.write(PC_BUF(p), 1 + (int)cw);
+  if (leader) tma_store_wait_all();  // shared memory must outlive the last stores' reads
 }
 
 static int ilog2_exact(uint32_t v) {
@@ -552,10 +915,26 @@ struct EpiMaps {
   CUtensorMap out, res1, res2;
 };
 
+#ifdef MTGEMM_PHASE_CLOCKS
+static long long* g_phase_buf = nullptr;
+#endif
+
+template <int BN, bool ALT>
+struct SchedCfg {
+  using type = TileCfg<BN>;
+  static constexpr auto kernel = mtgemm_kernel<BN>;
+};
 template <int BN>
+struct SchedCfg<BN, true> {
+  using type = AltCfg<BN>;
+  static constexpr auto kernel = mtgemm_alt_kernel<BN>;
+};
+
+template <int BN, bool ALT = false>
 static int launch(const b200svd_gemm_params* p, const CUtensorMap& tmA, const EpiMaps& em, const GemmDev& d,
                   cudaStream_t st) {
-  using Cfg = TileCfg<BN>;
+  using Cfg = typename SchedCfg<BN, ALT>::type;
+  constexpr auto kernel = SchedCfg<BN, ALT>::kernel;
   // weights [taps][n][k] -> TMA dims (k, n, taps)
   CUtensorMap tmB;
   uint64_t bd[3] = {p->k, p->n, p->taps};
@@ -563,6 +942,9 @@ static int launch(const b200svd_gemm_params* p, const CUtensorMap& tmA, const Ep
   uint32_t bb[3] = {64, (uint32_t)BN, 1};
   if (encode_tmap_bf16(&tmB, p->w_ptr, 3, bd, bs, bb)) return 1;
   GemmDev dd = d;
+#ifdef MTGEMM_PHASE_CLOCKS
+  dd.phase_buf = g_phase_buf;
+#endif
   dd.n_tiles = (p->n + BN - 1) / BN;
   // Ring depths.  Without residuals every byte past the fixed areas goes to A/B stages.  With residuals (bf16
   // output) stages are given up, down to MIN_STAGES, until the residual ring holds a whole tile's residual sub-tiles.
@@ -578,11 +960,11 @@ static int launch(const b200svd_gemm_params* p, const CUtensorMap& tmA, const Ep
   }
   dd.stages = (uint32_t)stages;
   dd.res_slots = (uint32_t)res_slots;
-  const int smem_bytes = stages * Cfg::STAGE_BYTES + res_slots * RES_SLOT_BYTES + FIXED_BYTES;
+  const int smem_bytes = stages * Cfg::STAGE_BYTES + res_slots * RES_SLOT_BYTES + Cfg::FIXED;
   const int slot = dev_slot();
   static bool attr_set[B200_MAX_DEVICES] = {};
   if (!attr_set[slot]) {
-    cudaError_t e = cudaFuncSetAttribute(mtgemm_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT);
+    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT);
     if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(mtgemm)");
     attr_set[slot] = true;
   }
@@ -594,7 +976,7 @@ static int launch(const b200svd_gemm_params* p, const CUtensorMap& tmA, const Ep
   }
   dd.total_tiles = (uint32_t)total;
   const uint32_t grid = (uint32_t)(total < (uint64_t)sm_count() ? total : (uint64_t)sm_count());
-  mtgemm_kernel<BN><<<grid, NUM_THREADS, smem_bytes, st>>>(tmA, tmB, em.out, em.res1, em.res2, dd);
+  kernel<<<grid, NUM_THREADS, smem_bytes, st>>>(tmA, tmB, em.out, em.res1, em.res2, dd);
   B200_CHECK_LAUNCH("mtgemm launch");
   return 0;
 }
@@ -602,7 +984,35 @@ static int launch(const b200svd_gemm_params* p, const CUtensorMap& tmA, const Ep
 // Kept for the C ABI: CTA-pair (cta_group::2) tiles do not exist on sm_90, every launch uses single-CTA tiles.
 static int g_pair_mode = 2;
 
+// Schedule choice, see b200svd_gemm_schedule in b200svd.h.  The alternating schedule pays for hiding the epilogue
+// with narrower tiles (about a third more bytes from L2 into shared memory per MMA at 128 against 256 columns), so
+// the rule keeps it to tiles whose MMAs are short enough for the epilogue to matter: taps x kblocks x 2 x BN tensor
+// core clocks per tile.
+static int g_schedule = 2;
+constexpr uint64_t ALT_MAX_TILE_MMA_CLOCKS = 20000;
+
+// N tile of the alternating schedule for a launch whose cooperative tile is `bn`, 0 if it has none.  A GEGLU launch
+// cannot change its tile: the weights are interleaved per tile.
+static int alt_tile(int bn, bool geglu) {
+  if (bn == 256 && !geglu) return 128;
+  return bn <= 160 ? bn : 0;
+}
+
 }  // namespace b200
+
+extern "C" int b200svd_gemm_schedule(int mode) {
+  const int prev = b200::g_schedule;
+  if (mode >= 0 && mode <= 2) b200::g_schedule = mode;
+  return prev;
+}
+
+#ifdef MTGEMM_PHASE_CLOCKS
+// Measuring build only: device buffer of [CTA][3 roles][8] int64 clock sums that every following launch adds to.
+extern "C" int b200svd_gemm_phase_buffer(void* buf) {
+  b200::g_phase_buf = reinterpret_cast<long long*>(buf);
+  return 0;
+}
+#endif
 
 extern "C" int b200svd_gemm_pair_mode(int mode) {
   const int prev = b200::g_pair_mode;
@@ -689,9 +1099,9 @@ extern "C" int b200svd_gemm(const b200svd_gemm_params* p, void* stream) {
   int bn = p->bn;
   if (p->act == B200SVD_ACT_GEGLU) {
     if (bn == 0) bn = 256;
-    if (bn != 256 || (p->n % 256) != 0) {
-      set_error("b200svd_gemm: GEGLU needs n (%u) divisible by 256 and the 256-wide tile (weights interleaved per tile)",
-                p->n);
+    if ((bn != 256 && bn != 128) || (p->n % (uint32_t)bn) != 0) {
+      set_error("b200svd_gemm: GEGLU needs the 128- or 256-wide tile its weights were interleaved for and n (%u) "
+                "divisible by it, got bn=%d", p->n, bn);
       return 1;
     }
   }
@@ -734,6 +1144,20 @@ extern "C" int b200svd_gemm(const b200svd_gemm_params* p, void* stream) {
   EpiMaps em;
   memset(&em, 0, sizeof(em));
   d.staged = !p->out_fp32 && n_out % 8 == 0;
+  int alt_bn = 0;
+  if (d.staged && p->gn_part == nullptr && g_schedule != 0) {
+    alt_bn = alt_tile(bn, p->act == B200SVD_ACT_GEGLU);
+    if (alt_bn != 0 && g_schedule == 2) {
+      // The 160-wide tile (N = 160, 320) measured slower alternating than cooperative (M 460800, K 1280, N 320 with a
+      // residual: 3.2 ms against 1.4 ms on an H100 at 700 W), so the rule leaves it cooperative; mode 1 still runs it.
+      if (alt_bn == 160) alt_bn = 0;
+    }
+    if (alt_bn != 0 && g_schedule == 2) {
+      const uint64_t tiles = m_tiles_all * ((p->n + alt_bn - 1) / alt_bn);
+      const uint64_t mma_clocks = (uint64_t)d.taps * d.kblocks * 2 * alt_bn;
+      if (tiles < 2 * (uint64_t)sm_count() || mma_clocks >= ALT_MAX_TILE_MMA_CLOCKS) alt_bn = 0;
+    }
+  }
   if (d.staged) {
     for (int i = 0; i < 3; ++i) {
       if (p->out_rs[i] <= 0) {
@@ -749,8 +1173,10 @@ extern "C" int b200svd_gemm(const b200svd_gemm_params* p, void* stream) {
     // each consumer warpgroup stores its 64 rows: the row box halved in its outermost non-unit dimension
     uint32_t ob[4] = {(uint32_t)SUB_W, p->m_box[0], p->m_box[1], p->m_box[2]};
     const int hd = p->m_box[2] > 1 ? 2 : (p->m_box[1] > 1 ? 1 : 0);
-    ob[1 + hd] /= 2;
-    d.wg_off[hd] = ob[1 + hd];
+    if (alt_bn == 0) {  // the alternating schedule stores the whole row box
+      ob[1 + hd] /= 2;
+      d.wg_off[hd] = ob[1 + hd];
+    }
     uint64_t os[3];
     row_strides(p->ldo, os);
     if (encode_tmap_bf16_sw64(&em.out, p->out, 4, od, os, ob)) return 1;
@@ -768,6 +1194,13 @@ extern "C" int b200svd_gemm(const b200svd_gemm_params* p, void* stream) {
   CUtensorMap tmA;
   if (encode_tmap_bf16(&tmA, p->a_ptr, 5, p->a_dims, p->a_strides, p->a_box)) return 1;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  switch (alt_bn) {
+    case 0: break;
+    case 32: return launch<32, true>(p, tmA, em, d, st);
+    case 64: return launch<64, true>(p, tmA, em, d, st);
+    case 128: return launch<128, true>(p, tmA, em, d, st);
+    case 160: return launch<160, true>(p, tmA, em, d, st);
+  }
   switch (bn) {
     case 32: return launch<32>(p, tmA, em, d, st);
     case 64: return launch<64>(p, tmA, em, d, st);

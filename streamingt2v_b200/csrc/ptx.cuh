@@ -126,6 +126,16 @@ __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
 
+// monotonic counters in shared memory, published by one thread and polled by others of the CTA
+__device__ __forceinline__ void st_release_shared(uint32_t* p, uint32_t v) {
+  asm volatile("st.release.cta.shared::cta.u32 [%0], %1;" ::"r"(smem_u32(p)), "r"(v) : "memory");
+}
+__device__ __forceinline__ uint32_t ld_acquire_shared(const uint32_t* p) {
+  uint32_t v;
+  asm volatile("ld.acquire.cta.shared::cta.u32 %0, [%1];" : "=r"(v) : "r"(smem_u32(p)) : "memory");
+  return v;
+}
+
 __device__ __forceinline__ void named_bar_arrive(int id, int nthreads) {
   asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }

@@ -129,7 +129,8 @@ class _NetWeights:
                         return P.pack_linear(w, device)
 
                     def geglu(q):
-                        return P.pack_geglu(sd[q + ".weight"], sd[q + ".bias"], device)
+                        # K <= 1280: short tiles, packed for the GEMM's alternating schedule
+                        return P.pack_geglu(sd[q + ".weight"], sd[q + ".bias"], device, bn=128)
 
                     d = dict(
                         ch=c, heads=layer.heads,

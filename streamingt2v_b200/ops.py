@@ -30,6 +30,13 @@ def gemm_pair_mode(mode: int = -1) -> int:
     return int(_lib.load().b200svd_gemm_pair_mode(int(mode)))
 
 
+def gemm_schedule(mode: int = -1) -> int:
+    """Consumer schedule of the GEMM: 0 = cooperative everywhere, 1 = alternating wherever it exists, 2 = alternating
+    for launches of many short tiles (default); see b200svd_gemm_schedule.  Any other value only queries.  Returns
+    the previous mode.  The output does not depend on it."""
+    return int(_lib.load().b200svd_gemm_schedule(int(mode)))
+
+
 def flash_attn_variant(v: int = -1) -> int:
     """Records a softmax variant (3..5; kept for ABI compatibility: the sm_90 kernel has one softmax organisation).
     Any other value only queries.  Returns the previous variant."""

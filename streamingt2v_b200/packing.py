@@ -52,13 +52,18 @@ def geglu_tile(n2: int) -> int:
     return 256
 
 
-def pack_geglu(w: torch.Tensor, b: torch.Tensor, device):
+def pack_geglu(w: torch.Tensor, b: torch.Tensor, device, bn: int = 0):
     """GEGLU proj weight [2F, K] (rows [0,F) = value, [F,2F) = gate; attention.py:94-101) -> rows interleaved per
     N tile: tile j holds value rows [j*h, (j+1)*h) followed by the matching gate rows, h = bn/2.
+    bn: the N tile, 256 (0 = geglu_tile's choice) or 128.  The 128-wide tile lets the GEMM alternate whole tiles
+    between its consumer warpgroups, which suits short-K projections; the output is the same either way.
     Returns (w_packed [1, 2F, K] bf16, bias_packed [2F] fp32, bn)."""
     n2, k = w.shape
     f = n2 // 2
-    bn = geglu_tile(n2)
+    if bn == 0:
+        bn = geglu_tile(n2)
+    if bn not in (128, 256) or n2 % bn != 0:
+        raise ValueError(f"GEGLU width {n2} must be a multiple of its N tile {bn} (128 or 256)")
     h = bn // 2
     idx = []
     for j in range(n2 // bn):
