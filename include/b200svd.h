@@ -108,6 +108,28 @@ int b200svd_gemm_pair_mode(int mode);
  * Both schedules give bitwise the same output. */
 int b200svd_gemm_schedule(int mode);
 
+/* Epilogue bodies of bf16 outputs written by TMA stores (no reference counterpart).  The combinations of activation,
+ * bias, per-frame vector and residuals that the networks launch are compiled as branch-free bodies, chosen once per
+ * tile; every other launch (another combination, gn_part, fp32 output, an output width that is not a multiple of 8)
+ * runs the generic body, which tests each of them per element.  Both give bitwise the same output. */
+enum {
+  B200SVD_EPI_GENERIC = 0,
+  B200SVD_EPI_PLAIN = 1,          /* no bias, nothing else */
+  B200SVD_EPI_BIAS = 2,
+  B200SVD_EPI_BIAS_RES1 = 3,
+  B200SVD_EPI_BIAS_RES1_FVEC = 4,
+  B200SVD_EPI_BIAS_FVEC = 5,
+  B200SVD_EPI_BIAS_GEGLU = 6,
+  B200SVD_EPI_BIAS_RES2 = 7,      /* res1 and res2 */
+  B200SVD_EPI_BIAS_SILU = 8,
+  B200SVD_EPI_BIAS_GELU = 9
+};
+/* 0 = the generic body everywhere, 1 (default) = a compiled kind wherever one exists; returns the previous mode,
+ * other values only query. */
+int b200svd_gemm_epilogue(int mode);
+/* The B200SVD_EPI_* body b200svd_gemm would run for these parameters under the current mode, without launching. */
+int b200svd_gemm_epilogue_kind(const b200svd_gemm_params* p);
+
 /* ---- FlashAttention forward, head dim 64 (wgmma + TMA) -----------------------------------------------------
  * Spatial self-attention core of BasicTransformerBlock.attn1 (attention.py:320-351 SDPA / :427-446 xformers).
  * qkv: [(n s), ldqkv] bf16, columns [q | k | v] each heads*64 wide (output of the fused QKV projection);

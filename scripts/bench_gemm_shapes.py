@@ -3,7 +3,8 @@
 
     python scripts/bench_gemm_shapes.py [--out FILE] [--no-phases]
 
-For each shape and schedule (0 = cooperative, 2 = the default rule): warm-up, CUDA events over enough launches for
+For each shape, schedule (0 = cooperative, 2 = the default rule) and epilogue body (0 = generic, 1 = the compile-time
+kind, ops.gemm_epilogue): warm-up, CUDA events over enough launches for
 at least 0.2 s, achieved TFLOP/s and GB/s from the shape (the formulas of ops.gemm_raw), and the bound that applies
 against the H100 SXM data sheet (989 TFLOP/s dense bf16, 3.35 TB/s) -- data-sheet figures, not reached ones.  The
 card's name and power limit are read in the same run.
@@ -38,6 +39,9 @@ def shapes():
         out += [(f"geglu {h}x{w} K{c}", "geglu", m, c, 8 * c),
                 (f"qkv {h}x{w} K{c}", "linear", m, c, 3 * c),
                 (f"residual linear {h}x{w} K{c}", "linear_res", m, c, c),
+                (f"fvec + res1 linear {h}x{w} K{c}", "linear_res_fvec", m, c, c),
+                (f"ff-out 2 residuals, s_acc {h}x{w} K{4 * c}", "linear_res2", m, 4 * c, c),
+                (f"conv3x3 + fvec {h}x{w} C{c}", "conv3x3_fvec", (FRAMES, h, w), c, c),
                 (f"ff-out {h}x{w} K{4 * c}", "linear_res", m, 4 * c, c),
                 (f"conv3x3 {h}x{w} C{c}", "conv3x3", (FRAMES, h, w), c, c),
                 (f"tconv(3,1,1) {h}x{w} C{c}", "tconv3", (2, 25, h * w), c, c)]
@@ -86,16 +90,25 @@ def main():
             packs = {0: packing.pack_geglu(w, bias.cpu(), dev), 2: packing.pack_geglu(w, bias.cpu(), dev, bn=128)}
             run = lambda s, x=x, packs=packs: ops.linear(x, packs[s][0], packs[s][1], act=ops.ACT_GEGLU, bn=packs[s][2])
             rows, taps, n_out, nres = m, 1, n // 2, 0
-        elif kind in ("linear", "linear_res"):
+        elif kind.startswith("linear"):
             x = rnd((m, k))
             w = packing.pack_linear(torch.randn((n, k), generator=g) * k ** -0.5, dev)
-            res = rnd((m, n)) if kind == "linear_res" else None
-            run = lambda s, x=x, w=w, bias=bias, res=res: ops.linear(x, w, bias, res1=res)
-            rows, taps, n_out, nres = m, 1, n, int(res is not None)
-        elif kind == "conv3x3":
+            kw = {}
+            if kind != "linear":
+                kw.update(res1=rnd((m, n)))
+            if kind == "linear_res2":
+                kw.update(res2=rnd((m, n)), s2=0.5, s_acc=0.7)
+            if kind == "linear_res_fvec":
+                kw.update(fvec=rnd((FRAMES, n), 1.0, torch.float32), rows_per_frame=m // FRAMES)
+            run = lambda s, x=x, w=w, bias=bias, kw=kw: ops.linear(x, w, bias, **kw)
+            rows, taps, n_out, nres = m, 1, n, ("res1" in kw) + ("res2" in kw)
+        elif kind in ("conv3x3", "conv3x3_fvec"):
             x = rnd((*m, k))
             w = packing.pack_conv3x3(torch.randn((n, k, 3, 3), generator=g) * (9 * k) ** -0.5, dev)
-            run = lambda s, x=x, w=w, bias=bias: ops.conv3x3(x, w, bias)
+            kw = {}
+            if kind == "conv3x3_fvec":
+                kw.update(fvec=rnd((m[0], n), 1.0, torch.float32), rows_per_frame=m[1] * m[2])
+            run = lambda s, x=x, w=w, bias=bias, kw=kw: ops.conv3x3(x, w, bias, **kw)
             rows, taps, n_out, nres = m[0] * m[1] * m[2], 9, n, 0
         else:
             x = rnd((*m, k))
@@ -107,11 +120,12 @@ def main():
         nbytes = 2.0 * rows * k + 2.0 * taps * n * k + 2.0 * rows * n_out * (1 + nres)
         cases.append((name, run, flops, nbytes))
 
-    prev = ops.gemm_schedule(-1)
-    lines.append(f"{'shape':34s} {'sched':5s} {'ms':>8s} {'TFLOP/s':>8s} {'GB/s':>7s}  bound (data sheet)      share")
+    prev, prev_epi = ops.gemm_schedule(-1), ops.gemm_epilogue(-1)
+    lines.append(f"{'shape':44s} {'sched':5s} {'epi':3s} {'ms':>8s} {'TFLOP/s':>8s} {'GB/s':>7s}  bound (data sheet)      share")
     for name, run, flops, nbytes in cases:
-        for sched in (0, 2):
+        for sched, epi in ((0, 0), (0, 1), (2, 0), (2, 1)):
             ops.gemm_schedule(sched)
+            ops.gemm_epilogue(epi)
             for _ in range(3):
                 run(sched)
             torch.cuda.synchronize()
@@ -128,9 +142,10 @@ def main():
             t = ms / reps
             t_ops, t_bytes = flops / PEAK_TFLOPS / 1e9, nbytes / PEAK_GBS / 1e6
             bound = "operations" if t_ops >= t_bytes else "bytes"
-            lines.append(f"{name:34s} {sched:5d} {t:8.3f} {flops / t / 1e9:8.1f} {nbytes / t / 1e6:7.0f}  "
+            lines.append(f"{name:44s} {sched:5d} {epi:3d} {t:8.3f} {flops / t / 1e9:8.1f} {nbytes / t / 1e6:7.0f}  "
                          f"{bound:10s} {max(t_ops, t_bytes):7.3f} ms  {max(t_ops, t_bytes) / t:5.1%}")
     ops.gemm_schedule(prev)
+    ops.gemm_epilogue(prev_epi)
 
     if not args.no_phases:
         with tempfile.TemporaryDirectory() as tmp:
@@ -145,10 +160,11 @@ def main():
             lib.b200svd_gemm_phase_buffer(C.c_void_p(buf.data_ptr()))
             lines.append("")
             lines.append("phase shares of the thread's lifetime (clock64, one launch, mean over CTAs)")
-            lines.append(f"{'shape':34s} {'sched':5s} role      " + " ".join(f"{p:>10s}" for p in PHASES))
+            lines.append(f"{'shape':44s} {'sched':5s} {'epi':3s} role      " + " ".join(f"{p:>10s}" for p in PHASES))
             for name, run, _, _ in cases:
-                for sched in (0, 2):
+                for sched, epi in ((0, 0), (0, 1), (2, 0), (2, 1)):
                     ops.gemm_schedule(sched)
+                    ops.gemm_epilogue(epi)
                     run(sched)
                     torch.cuda.synchronize()
                     buf.zero_()
@@ -160,8 +176,10 @@ def main():
                         if tot == 0:
                             continue
                         sh = [b[:, role, i].sum().item() / tot for i in range(6)]
-                        lines.append(f"{name:34s} {sched:5d} {rname:9s} " + " ".join(f"{v:10.1%}" for v in sh))
+                        lines.append(f"{name:44s} {sched:5d} {epi:3d} {rname:9s} " + " ".join(f"{v:10.1%}" for v in sh))
             lib.b200svd_gemm_phase_buffer(C.c_void_p(0))
+            ops.gemm_schedule(prev)
+            ops.gemm_epilogue(prev_epi)
     text = "\n".join(lines)
     print(text)
     if args.out:

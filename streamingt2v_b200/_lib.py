@@ -15,6 +15,9 @@ LIB_PATH = Path(__file__).resolve().parent / "libb200svd.so"
 
 MAX_TAPS = 12
 ACT_NONE, ACT_SILU, ACT_GELU, ACT_GEGLU = 0, 1, 2, 3
+# B200SVD_EPI_*: compile-time epilogue kinds of the GEMM, 0 = the generic body
+(EPI_GENERIC, EPI_PLAIN, EPI_BIAS, EPI_BIAS_RES1, EPI_BIAS_RES1_FVEC, EPI_BIAS_FVEC, EPI_BIAS_GEGLU, EPI_BIAS_RES2,
+ EPI_BIAS_SILU, EPI_BIAS_GELU) = range(10)
 
 
 class GemmParams(C.Structure):
@@ -95,6 +98,8 @@ _P, _I64, _I, _F = C.c_void_p, C.c_int64, C.c_int, C.c_float
 PROTOTYPES = {
     "b200svd_gemm": [C.POINTER(GemmParams), _P],
     "b200svd_gemm_schedule": [_I],                      # returns the previous schedule, not a status
+    "b200svd_gemm_epilogue": [_I],                      # returns the previous mode
+    "b200svd_gemm_epilogue_kind": [C.POINTER(GemmParams)],  # returns a B200SVD_EPI_* id
     "b200svd_flash_attn": [_P, _I64, _P, _I64, _I, _I, _I, _F, _P],
     "b200svd_flash_attn_d80": [_P, _I64, _P, _I64, _I, _I, _I, _F, _P],
     "b200svd_clip_preprocess": [_P, _I, _I, _I, _P, _I64, _P, _I, _P, _I, _P],

@@ -67,6 +67,7 @@ struct GemmDev {
   int64_t gn_ld;
   uint32_t gn_rows;
   int32_t staged;      // bf16 output through shared memory and TMA stores (else straight from registers)
+  int32_t epi_kind;    // B200SVD_EPI_*: the compile-time epilogue body of a staged launch, 0 = the generic one
   uint32_t stages;     // depth of the A/B stage ring
   uint32_t res_slots;  // depth of the residual ring (bf16 outputs with residuals, else 0)
   uint32_t wg_off[3];  // row-box origin of the second consumer warpgroup's 64 rows (bf16 output stores)
@@ -237,6 +238,125 @@ __device__ __forceinline__ uint32_t sw64_off(uint32_t row, uint32_t ch, uint32_t
   return row * 64u + ((ch ^ ((row >> 1) & 3u)) << 4) + cp * 4u;
 }
 
+// ---- compile-time epilogue kinds of the staged bf16 output ----
+// The generic epilogue tests activation, bias, per-frame vector and residuals per element; those tests, and the global
+// loads sitting between them, are what a consumer warp spends its epilogue on.  The combinations the network launches
+// (b200svd_gemm_epilogue_kind) are compiled as branch-free bodies instead: one switch per tile picks the body.  Per
+// element the arithmetic is that of the generic body, operation for operation, so the output is bitwise the same.
+template <int ACT_, bool BIAS_, bool FVEC_, int NRES_>
+struct Epi {
+  static constexpr int ACT = ACT_;
+  static constexpr bool BIAS = BIAS_, FVEC = FVEC_, GEGLU = ACT_ == B200SVD_ACT_GEGLU;
+  static constexpr int NRES = NRES_;
+};
+// X(kind id, activation, bias, per-frame vector, residuals): what the two kernels instantiate
+#define MTGEMM_EPI_KINDS(X)                                    \
+  X(B200SVD_EPI_PLAIN, B200SVD_ACT_NONE, false, false, 0)      \
+  X(B200SVD_EPI_BIAS, B200SVD_ACT_NONE, true, false, 0)        \
+  X(B200SVD_EPI_BIAS_RES1, B200SVD_ACT_NONE, true, false, 1)   \
+  X(B200SVD_EPI_BIAS_RES1_FVEC, B200SVD_ACT_NONE, true, true, 1) \
+  X(B200SVD_EPI_BIAS_FVEC, B200SVD_ACT_NONE, true, true, 0)    \
+  X(B200SVD_EPI_BIAS_GEGLU, B200SVD_ACT_GEGLU, true, false, 0) \
+  X(B200SVD_EPI_BIAS_RES2, B200SVD_ACT_NONE, true, false, 2)   \
+  X(B200SVD_EPI_BIAS_SILU, B200SVD_ACT_SILU, true, false, 0)   \
+  X(B200SVD_EPI_BIAS_GELU, B200SVD_ACT_GELU, true, false, 0)
+
+// epi_act with the activation known at compile time
+template <int ACT>
+__device__ __forceinline__ float epi_act_kind(float s_acc, float v, float g) {
+  if constexpr (ACT == B200SVD_ACT_SILU) v = silu_fast(v);
+  if constexpr (ACT == B200SVD_ACT_GELU) v = gelu_fast(v);
+  if constexpr (ACT == B200SVD_ACT_GEGLU) v = __fmul_rn(v, gelu_fast(g));
+  return __fmul_rn(v, s_acc);
+}
+
+// What a consumer thread knows about its tile
+struct EpiTile {
+  uint32_t n0, otile0, n_out;  // first GEMM column, first output column, output width
+  uint32_t mb1, mb2, mb3;      // row box origin
+};
+
+// Bias and GEGLU gate bias of the thread's 8 columns of sub-tile c, loaded in one batch ahead of the residual waits
+// and the arithmetic.  Columns past the output width read nothing.
+template <int BN, class E>
+__device__ __forceinline__ void epi_load_bias(const GemmDev& p, const EpiTile& t, int c, uint32_t cq, float (&bv)[4][2],
+                                              float (&gbv)[4][2]) {
+  if constexpr (E::BIAS) {
+#pragma unroll
+    for (int jj = 0; jj < 4; ++jj) {
+      const uint32_t tcol = (uint32_t)(8 * (4 * c + jj)) + 2 * cq;
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        bv[jj][e] = t.otile0 + tcol + e < t.n_out ? __ldg(p.bias + t.n0 + tcol + e) : 0.f;
+        if constexpr (E::GEGLU) gbv[jj][e] = __ldg(p.bias + t.n0 + BN / 2 + tcol + e);  // n is a multiple of BN
+      }
+    }
+  }
+}
+
+// One 64-row half of sub-tile c: the thread's rows rbase and rbase + 8 (of the 64), 8 columns each, from the m64nBN
+// accumulator fragment `acc` to the staging buffer `stg`; r1s / r2s are the residual sub-tiles of the same 64 rows.
+// fv[h] is the per-frame row of row h (any readable row if the row is outside the output: it is never stored); the
+// half's 16 per-frame values are loaded in one batch ahead of the arithmetic.
+// Order per element: bias, per-frame, gate bias, activation, s_acc, res1, res2, round.
+template <int BN, class E>
+__device__ __forceinline__ void epi_stage_half(const GemmDev& p, const EpiTile& t, const float (&acc)[BN / 2], int c,
+                                               uint32_t rbase, uint32_t cq, uint8_t* stg, const uint8_t* r1s,
+                                               const uint8_t* r2s, const float (&bv)[4][2], const float (&gbv)[4][2],
+                                               const float* const (&fv)[2]) {
+  constexpr int NJ = BN / 8;
+  float fvv[2][4][2];
+  if constexpr (E::FVEC) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int jj = 0; jj < 4; ++jj) {
+        const uint32_t ocol = t.otile0 + (uint32_t)(8 * (4 * c + jj)) + 2 * cq;
+#pragma unroll
+        for (int e = 0; e < 2; ++e) fvv[h][jj][e] = ocol + e < t.n_out ? __ldg(fv[h] + ocol + e) : 0.f;
+      }
+  }
+#pragma unroll
+  for (int jj = 0; jj < 4; ++jj) {
+    const int j = 4 * c + jj;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const uint32_t off = sw64_off(rbase + 8u * h, (uint32_t)jj, cq);
+      float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+      float g0 = 0.f, g1 = 0.f;
+      if constexpr (E::BIAS) {
+        v0 += bv[jj][0];
+        v1 += bv[jj][1];
+      }
+      if constexpr (E::FVEC) {
+        v0 += fvv[h][jj][0];
+        v1 += fvv[h][jj][1];
+      }
+      if constexpr (E::GEGLU) {
+        g0 = acc[4 * (j + NJ / 2) + 2 * h];
+        g1 = acc[4 * (j + NJ / 2) + 2 * h + 1];
+        if constexpr (E::BIAS) {
+          g0 += gbv[jj][0];
+          g1 += gbv[jj][1];
+        }
+      }
+      v0 = epi_act_kind<E::ACT>(p.s_acc, v0, g0);
+      v1 = epi_act_kind<E::ACT>(p.s_acc, v1, g1);
+      if constexpr (E::NRES >= 1) {
+        const uint32_t w = *reinterpret_cast<const uint32_t*>(r1s + off);
+        v0 = __fmaf_rn(p.s1, bf16_lo(w), v0);
+        v1 = __fmaf_rn(p.s1, bf16_hi(w), v1);
+      }
+      if constexpr (E::NRES >= 2) {
+        const uint32_t w = *reinterpret_cast<const uint32_t*>(r2s + off);
+        v0 = __fmaf_rn(p.s2, bf16_lo(w), v0);
+        v1 = __fmaf_rn(p.s2, bf16_hi(w), v1);
+      }
+      *reinterpret_cast<uint32_t*>(stg + off) = pack_bf16x2(v0, v1);
+    }
+  }
+}
+
 // TMA producer of the A/B stage ring (one thread): the CTA's tiles in order, taps and K blocks of each.  Both
 // schedules run it unchanged; the ring is what orders the consumers.
 template <int BN>
@@ -304,6 +424,114 @@ __device__ __forceinline__ void produce_residuals(const GemmDev& p, const CUtens
         }
       }
     }
+  }
+}
+
+// The staged bf16 epilogue of one tile on the cooperative schedule for epilogue kind E: the sub-tile loop of
+// mtgemm_kernel with the same waits, barrier and store order, the element loop replaced by epi_stage_half.
+template <int BN, class E>
+__device__ __forceinline__ void coop_epilogue_kind(const GemmDev& p, const CUtensorMap* tmO, const EpiTile& t,
+                                                   const float (&acc)[BN / 2], uint8_t* stg_smem,
+                                                   const uint8_t* res_smem, uint64_t* res_full, uint64_t* res_empty,
+                                                   uint32_t rslots, uint32_t& rslot, uint32_t& rph, uint32_t& stg_it,
+                                                   int cw, uint32_t rbase, uint32_t cq, bool leader,
+                                                   const float* const (&fv)[2], PhaseClock& pc) {
+  constexpr int NSUB = (E::GEGLU ? BN / 2 : BN) / SUB_W;  // gate columns are consumed with their value columns
+#pragma unroll
+  for (int c = 0; c < NSUB; ++c) {
+    if (t.otile0 + (uint32_t)(c * SUB_W) >= t.n_out) break;
+    uint8_t* stg = stg_smem + (cw * STG_SLOTS + (stg_it & 1)) * STG_SLOT_BYTES;
+    float bv[4][2], gbv[4][2];
+    epi_load_bias<BN, E>(p, t, c, cq, bv, gbv);
+    const uint8_t* r1s = res_smem;
+    const uint8_t* r2s = res_smem;
+    uint32_t r1slot = 0, r2slot = 0;
+    pc.mark(PC_EPI);
+    if constexpr (E::NRES >= 1) {
+      r1slot = rslot;
+      mbar_wait(&res_full[rslot], rph);
+      r1s = res_smem + rslot * RES_SLOT_BYTES + cw * STG_SLOT_BYTES;
+      if (++rslot == rslots) {
+        rslot = 0;
+        rph ^= 1;
+      }
+    }
+    if constexpr (E::NRES >= 2) {
+      r2slot = rslot;
+      mbar_wait(&res_full[rslot], rph);
+      r2s = res_smem + rslot * RES_SLOT_BYTES + cw * STG_SLOT_BYTES;
+      if (++rslot == rslots) {
+        rslot = 0;
+        rph ^= 1;
+      }
+    }
+    pc.mark(PC_RES_WAIT);
+    epi_stage_half<BN, E>(p, t, acc, c, rbase, cq, stg, r1s, r2s, bv, gbv, fv);
+    fence_proxy_async_smem();  // the staged values are read by the TMA store (async proxy)
+    // the store issued one sub-tile ago has read the other staging buffer: it may be refilled next sub-tile
+    pc.mark(PC_EPI);
+    if (leader) tma_store_wait_read0();
+    named_bar_sync(5 + cw, 128);
+    pc.mark(PC_STORE_WAIT);
+    if (leader) {
+      if constexpr (E::NRES >= 1) mbar_arrive(&res_empty[r1slot]);
+      if constexpr (E::NRES >= 2) mbar_arrive(&res_empty[r2slot]);
+      tma_store_4d(tmO, stg, (int)(t.otile0 + c * SUB_W), (int)(t.mb1 + (cw ? p.wg_off[0] : 0u)),
+                   (int)(t.mb2 + (cw ? p.wg_off[1] : 0u)), (int)(t.mb3 + (cw ? p.wg_off[2] : 0u)));
+      tma_store_commit();
+    }
+    ++stg_it;
+  }
+}
+
+// The same for the alternating schedule: the warpgroup holds both 64-row halves of the tile.
+template <int BN, class E>
+__device__ __forceinline__ void alt_epilogue_kind(const GemmDev& p, const CUtensorMap* tmO, const EpiTile& t,
+                                                  const float (&acc0)[BN / 2], const float (&acc1)[BN / 2],
+                                                  uint8_t* stg_smem, const uint8_t* res_smem, uint64_t* res_full,
+                                                  uint64_t* res_empty, uint32_t rslots, RingPos& rr, uint32_t& stg_it,
+                                                  uint32_t cw, uint32_t rbase, uint32_t cq, bool leader,
+                                                  const float* const (&fv)[2][2], PhaseClock& pc) {
+  constexpr int NSUB = (E::GEGLU ? BN / 2 : BN) / SUB_W;
+  constexpr uint32_t HALF = 64 * SUB_W * 2;  // bytes of a 64-row half of a sub-tile; the swizzle repeats every 8 rows
+#pragma unroll
+  for (int c = 0; c < NSUB; ++c) {
+    if (t.otile0 + (uint32_t)(c * SUB_W) >= t.n_out) break;
+    uint8_t* stg = stg_smem + (cw * STG_SLOTS + (stg_it & 1)) * ALT_STG_SLOT_BYTES;
+    float bv[4][2], gbv[4][2];
+    epi_load_bias<BN, E>(p, t, c, cq, bv, gbv);
+    const uint8_t* r1s = res_smem;
+    const uint8_t* r2s = res_smem;
+    uint32_t r1slot = 0, r2slot = 0;
+    pc.mark(PC_EPI);
+    if constexpr (E::NRES >= 1) {
+      r1slot = rr.idx;
+      mbar_wait(&res_full[rr.idx], rr.phase);
+      r1s = res_smem + rr.idx * RES_SLOT_BYTES;
+      ring_step(rr, rslots);
+    }
+    if constexpr (E::NRES >= 2) {
+      r2slot = rr.idx;
+      mbar_wait(&res_full[rr.idx], rr.phase);
+      r2s = res_smem + rr.idx * RES_SLOT_BYTES;
+      ring_step(rr, rslots);
+    }
+    pc.mark(PC_RES_WAIT);
+    epi_stage_half<BN, E>(p, t, acc0, c, rbase, cq, stg, r1s, r2s, bv, gbv, fv[0]);
+    epi_stage_half<BN, E>(p, t, acc1, c, rbase, cq, stg + HALF, r1s + HALF, r2s + HALF, bv, gbv, fv[1]);
+    fence_proxy_async_smem();  // the staged values are read by the TMA store (async proxy)
+    pc.mark(PC_EPI);
+    // the store issued one sub-tile ago has read the other staging buffer: it may be refilled next sub-tile
+    if (leader) tma_store_wait_read0();
+    named_bar_sync(5 + (int)cw, 128);
+    pc.mark(PC_STORE_WAIT);
+    if (leader) {
+      if constexpr (E::NRES >= 1) mbar_arrive(&res_empty[r1slot]);
+      if constexpr (E::NRES >= 2) mbar_arrive(&res_empty[r2slot]);
+      tma_store_4d(tmO, stg, (int)(t.otile0 + c * SUB_W), (int)t.mb1, (int)t.mb2, (int)t.mb3);  // the tile's row box
+      tma_store_commit();
+    }
+    ++stg_it;
   }
 }
 
@@ -428,6 +656,24 @@ mtgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
                                               : nullptr;
     }
     constexpr int NJ = BN / 8;
+    if (p.epi_kind != B200SVD_EPI_GENERIC) {
+      // ----- staged bf16 output, epilogue kind known at compile time (launch-uniform: one switch per tile) -----
+      const EpiTile et = {n0, otile0, n_out, mb1, mb2, mb3};
+      const float* const fvk[2] = {fv[0] != nullptr ? fv[0] : p.fvec, fv[1] != nullptr ? fv[1] : p.fvec};
+      const uint32_t rbase = (uint32_t)(16 * wl + rq);
+      switch (p.epi_kind) {
+#define MTGEMM_CASE(ID, ACT, BIAS, FVEC, NRES)                                                                    \
+  case ID:                                                                                                        \
+    if constexpr (ACT != B200SVD_ACT_GEGLU || BN == 128 || BN == 256)                                             \
+      coop_epilogue_kind<BN, Epi<ACT, BIAS, FVEC, NRES>>(p, &tmO, et, acc, stg_smem, res_smem, res_full,          \
+                                                         res_empty, rslots, rslot, rph, stg_it, cw, rbase,        \
+                                                         (uint32_t)cq, leader, fvk, pc);                          \
+    break;
+        MTGEMM_EPI_KINDS(MTGEMM_CASE)
+#undef MTGEMM_CASE
+      }
+      continue;
+    }
     if (p.staged) {
       // ----- bf16 output: 32-column sub-tiles staged in shared memory (SWIZZLE_64B, conflict-free fragment
       // writes), written by one TMA store per warpgroup and sub-tile; residuals come from the TMA-fed ring -----
@@ -804,6 +1050,30 @@ mtgemm_alt_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       }
       pc.mark(PC_RES_WAIT);
     }
+    if (BN <= 128 && p.epi_kind != B200SVD_EPI_GENERIC) {
+      // ----- epilogue kind known at compile time (launch-uniform: one switch per tile).  Not at BN = 160, whose 160
+      // accumulator registers leave the batched loads no room: that tile keeps the generic body -----
+      const EpiTile et = {n0, otile0, n_out, mb1, mb2, mb3};
+      const float* fvk[2][2];
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) fvk[hh][h] = fv[hh][h] != nullptr ? fv[hh][h] : p.fvec;
+      const uint32_t rbase = (uint32_t)(16 * wl + rq);
+      switch (p.epi_kind) {
+#define MTGEMM_CASE(ID, ACT, BIAS, FVEC, NRES)                                                                    \
+  case ID:                                                                                                        \
+    if constexpr (BN <= 128 && (ACT != B200SVD_ACT_GEGLU || BN == 128))                                           \
+      alt_epilogue_kind<BN, Epi<ACT, BIAS, FVEC, NRES>>(p, &tmO, et, acc0, acc1, stg_smem, res_smem, res_full,    \
+                                                        res_empty, rslots, rr, stg_it, cw, rbase, (uint32_t)cq,   \
+                                                        leader, fvk, pc);                                         \
+    break;
+        MTGEMM_EPI_KINDS(MTGEMM_CASE)
+#undef MTGEMM_CASE
+      }
+      if (leader && rslots != 0) st_release_shared(&tiles_done[2 + cw], t + 1);
+      continue;
+    }
 #pragma unroll
     for (int c = 0; c < Cfg::SUBTILES; ++c) {
       if (geglu && c >= Cfg::SUBTILES / 2) break;  // gate columns are consumed with their value columns
@@ -998,7 +1268,41 @@ static int alt_tile(int bn, bool geglu) {
   return bn <= 160 ? bn : 0;
 }
 
+// Epilogue body choice, see b200svd_gemm_epilogue in b200svd.h.
+static int g_epilogue = 1;
+
+// The compile-time epilogue kind of a launch (MTGEMM_EPI_KINDS), B200SVD_EPI_GENERIC if it has none: outputs that are
+// not staged bf16, GroupNorm partials, and every combination the list does not name.
+static int epilogue_kind(const b200svd_gemm_params* p) {
+  const uint32_t n_out = p->act == B200SVD_ACT_GEGLU ? p->n / 2 : p->n;
+  if (p->out_fp32 || n_out % 8 != 0 || p->gn_part != nullptr) return B200SVD_EPI_GENERIC;
+  const bool bias = p->bias != nullptr, fvec = p->fvec != nullptr;
+  const int nres = p->res1 == nullptr ? (p->res2 == nullptr ? 0 : -1) : (p->res2 == nullptr ? 1 : 2);
+  if (!bias) return p->act == B200SVD_ACT_NONE && !fvec && nres == 0 ? B200SVD_EPI_PLAIN : B200SVD_EPI_GENERIC;
+  switch (p->act) {
+    case B200SVD_ACT_NONE:
+      if (nres == 0) return fvec ? B200SVD_EPI_BIAS_FVEC : B200SVD_EPI_BIAS;
+      if (nres == 1) return fvec ? B200SVD_EPI_BIAS_RES1_FVEC : B200SVD_EPI_BIAS_RES1;
+      return nres == 2 && !fvec ? B200SVD_EPI_BIAS_RES2 : B200SVD_EPI_GENERIC;
+    case B200SVD_ACT_SILU: return !fvec && nres == 0 ? B200SVD_EPI_BIAS_SILU : B200SVD_EPI_GENERIC;
+    case B200SVD_ACT_GELU: return !fvec && nres == 0 ? B200SVD_EPI_BIAS_GELU : B200SVD_EPI_GENERIC;
+    case B200SVD_ACT_GEGLU: return !fvec && nres == 0 ? B200SVD_EPI_BIAS_GEGLU : B200SVD_EPI_GENERIC;
+    default: return B200SVD_EPI_GENERIC;
+  }
+}
+
 }  // namespace b200
+
+extern "C" int b200svd_gemm_epilogue(int mode) {
+  const int prev = b200::g_epilogue;
+  if (mode == 0 || mode == 1) b200::g_epilogue = mode;
+  return prev;
+}
+
+extern "C" int b200svd_gemm_epilogue_kind(const b200svd_gemm_params* p) {
+  if (p == nullptr || b200::g_epilogue == 0) return B200SVD_EPI_GENERIC;
+  return b200::epilogue_kind(p);
+}
 
 extern "C" int b200svd_gemm_schedule(int mode) {
   const int prev = b200::g_schedule;
@@ -1144,6 +1448,7 @@ extern "C" int b200svd_gemm(const b200svd_gemm_params* p, void* stream) {
   EpiMaps em;
   memset(&em, 0, sizeof(em));
   d.staged = !p->out_fp32 && n_out % 8 == 0;
+  d.epi_kind = g_epilogue != 0 ? epilogue_kind(p) : B200SVD_EPI_GENERIC;
   int alt_bn = 0;
   if (d.staged && p->gn_part == nullptr && g_schedule != 0) {
     alt_bn = alt_tile(bn, p->act == B200SVD_ACT_GEGLU);

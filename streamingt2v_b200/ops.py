@@ -37,6 +37,13 @@ def gemm_schedule(mode: int = -1) -> int:
     return int(_lib.load().b200svd_gemm_schedule(int(mode)))
 
 
+def gemm_epilogue(mode: int = -1) -> int:
+    """Epilogue body of the GEMM's staged bf16 outputs: 0 = the generic body everywhere, 1 = a compile-time kind
+    wherever one exists (default); see b200svd_gemm_epilogue.  Any other value only queries.  Returns the previous
+    mode.  The output does not depend on it."""
+    return int(_lib.load().b200svd_gemm_epilogue(int(mode)))
+
+
 def flash_attn_variant(v: int = -1) -> int:
     """Records a softmax variant (3..5; kept for ABI compatibility: the sm_90 kernel has one softmax organisation).
     Any other value only queries.  Returns the previous variant."""
@@ -182,7 +189,8 @@ def gemm_raw(*, a, a_dims, a_strides, a_box, w, n, k, taps, tap_off, m_ext, m_bo
         nbytes = 2.0 * rows * k + 2.0 * taps * n * k + (4.0 if out_fp32 else 2.0) * rows * n_out
         nbytes += 2.0 * rows * n_out * ((res1 is not None) + (res2 is not None))
         desc = (f"M{rows} K{k} N{n} taps{taps} act{act} res{(res1 is not None) + (res2 is not None)} "
-                f"fvec{int(fvec is not None)} f32{int(out_fp32)} box{tuple(int(b) for b in m_box)}")
+                f"fvec{int(fvec is not None)} f32{int(out_fp32)} box{tuple(int(b) for b in m_box)} "
+                f"epi{int(lib.b200svd_gemm_epilogue_kind(C.byref(p)))}")
         _prof_end(e0, ("mtgemm", desc), 2.0 * rows * k * n * taps, nbytes)
 
 
