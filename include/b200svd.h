@@ -258,6 +258,15 @@ int b200svd_ddim_blend_step(const float* noise, const float* lat, float* out, in
 int b200svd_frames_to_uint8(const float* x, void* out, int64_t n, int c, int64_t hw, float vmin, float vmax,
                             void* stream);
 
+/* ---- the 8-bit round trip of the first chunk ---------------------------------------------------------------------
+ * The first chunk of a request passes through 8-bit images before the later chunks condition on it: diffusers'
+ * postprocess_video(output_type="pil") then ToTensor() and `* 2.0 - 1` (code/diffusion_trainer/streaming_svd.py:390-393).
+ * Elementwise over n fp32 values in [-1, 1], each step one fp32 operation in this order:
+ *   v = clamp(x / 2 + 0.5, 0, 1);  q = round_half_to_even(v * 255);  out = (q / 255) * 2 - 1.
+ * The result lies on the 1/127.5 grid; unlike b200svd_frames_to_uint8 (which truncates, as torch2np does) it rounds.
+ * out may alias x. */
+int b200svd_frames_quantize(const float* x, float* out, int64_t n, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -122,6 +122,7 @@ PROTOTYPES = {
     "b200svd_sampler_step": [_P, _P, _P, _I64, _I64, _I, _P, _F, _F, _F, _F, _P],
     "b200svd_gn_stats_partials": [_P, _P, _I64, _I64, _I, _I64, _P, _P, _P, _P],
     "b200svd_frames_to_uint8": [_P, _P, _I64, _I, _I64, _F, _F, _P],
+    "b200svd_frames_quantize": [_P, _P, _I64, _P],
     "b200svd_ddim_blend_step": [_P, _P, _P, _I, _I, _I64, _I, _I, _I, _I, _I, _I, _F, _F, _F, _I, _P],
 }
 

@@ -625,3 +625,162 @@ def clip_visual_param_shapes(cfg: ClipVisionConfig) -> Dict[str, tuple]:
     _norm(d, "ln_post", w)
     d["proj"] = (w, cfg.output_dim)
     return d
+
+
+def clip_vision_config_from_hf(hcfg) -> ClipVisionConfig:
+    """ClipVisionConfig of a transformers `CLIPVisionConfig` (the `config` of `CLIPVisionModelWithProjection`, the
+    `image_encoder` of the SVD-XT checkpoint).  The tower computes erf GELU, so any other `hidden_act` is rejected."""
+    if hcfg.hidden_act != "gelu":
+        raise ValueError(f"hidden_act {hcfg.hidden_act!r}: the CLIP tower computes erf GELU ('gelu') only")
+    return ClipVisionConfig(image_size=hcfg.image_size, patch_size=hcfg.patch_size, width=hcfg.hidden_size,
+                            layers=hcfg.num_hidden_layers, heads=hcfg.num_attention_heads,
+                            mlp=hcfg.intermediate_size, output_dim=hcfg.projection_dim, eps=hcfg.layer_norm_eps)
+
+
+def _check_shapes(out: Dict[str, "torch.Tensor"], shapes: Dict[str, tuple], what: str):
+    if set(out) != set(shapes):
+        raise KeyError(f"{what}: mapped keys differ from the grammar: missing {sorted(set(shapes) - set(out))[:4]}, "
+                       f"extra {sorted(set(out) - set(shapes))[:4]}")
+    for k, t in out.items():
+        if tuple(t.shape) != tuple(shapes[k]):
+            raise ValueError(f"{what}: {k} has shape {tuple(t.shape)}, expected {shapes[k]}")
+
+
+def from_hf_clip_vision_state_dict(sd: Dict[str, "torch.Tensor"], cfg) -> Dict[str, "torch.Tensor"]:
+    """State dict of transformers' `CLIPVisionModelWithProjection` -> open_clip `visual` layout
+    (clip_visual_param_shapes) that B200ClipImageEncoder reads.  `cfg` is the model's transformers CLIPVisionConfig.
+
+    q/k/v_proj are concatenated into in_proj_weight / in_proj_bias (open_clip's nn.MultiheadAttention packs them in
+    that order), visual_projection.weight is stored transposed as `proj`, pre_layrnorm / post_layernorm become
+    ln_pre / ln_post and the embeddings are renamed.  `vision_model.embeddings.position_ids` (a buffer, not a weight)
+    is ignored; any other key left over is an error.  Restated from transformers' published CLIP modelling source;
+    the test suite runs transformers' own model on the renamed weights."""
+    import torch
+    ccfg = clip_vision_config_from_hf(cfg)
+    v = "vision_model."
+    out = {"conv1.weight": sd[v + "embeddings.patch_embedding.weight"],
+           "class_embedding": sd[v + "embeddings.class_embedding"],
+           "positional_embedding": sd[v + "embeddings.position_embedding.weight"],
+           "ln_pre.weight": sd[v + "pre_layrnorm.weight"], "ln_pre.bias": sd[v + "pre_layrnorm.bias"],
+           "ln_post.weight": sd[v + "post_layernorm.weight"], "ln_post.bias": sd[v + "post_layernorm.bias"],
+           "proj": sd["visual_projection.weight"].t().contiguous()}
+    used = {v + "embeddings.patch_embedding.weight", v + "embeddings.class_embedding",
+            v + "embeddings.position_embedding.weight", v + "pre_layrnorm.weight", v + "pre_layrnorm.bias",
+            v + "post_layernorm.weight", v + "post_layernorm.bias", "visual_projection.weight"}
+    for i in range(ccfg.layers):
+        b, h = f"transformer.resblocks.{i}", f"{v}encoder.layers.{i}"
+        for leaf in ("weight", "bias"):
+            qkv = [f"{h}.self_attn.{n}_proj.{leaf}" for n in "qkv"]
+            out[f"{b}.attn.in_proj_{leaf}"] = torch.cat([sd[k] for k in qkv], 0)
+            used.update(qkv)
+            for a, o in (("attn.out_proj", "self_attn.out_proj"), ("ln_1", "layer_norm1"), ("ln_2", "layer_norm2"),
+                         ("mlp.c_fc", "mlp.fc1"), ("mlp.c_proj", "mlp.fc2")):
+                out[f"{b}.{a}.{leaf}"] = sd[f"{h}.{o}.{leaf}"]
+                used.add(f"{h}.{o}.{leaf}")
+    extra = sorted(k for k in sd if k not in used and not k.endswith("position_ids"))
+    if extra:
+        raise KeyError(f"{len(extra)} CLIP keys without an open_clip counterpart, e.g. {extra[:4]}")
+    _check_shapes(out, clip_visual_param_shapes(ccfg), "CLIP vision")
+    return out
+
+
+# --------------------------------------------------------------------------------------------------------------
+# diffusers weight layout of the SVD-XT VAE (AutoencoderKLTemporalDecoder: SD-VAE Encoder + quant_conv, TemporalDecoder)
+# --------------------------------------------------------------------------------------------------------------
+_VAE_RES_MAP = (("norm1", "norm1"), ("conv1", "conv1"), ("norm2", "norm2"), ("conv2", "conv2"),
+                ("nin_shortcut", "conv_shortcut"))
+# decoder resnets are SpatioTemporalResBlocks: the spatial ResnetBlock2D sits under spatial_res_block
+_VAE_VIDEO_RES_MAP = tuple((a, "spatial_res_block." + b) for a, b in _VAE_RES_MAP) + (
+    ("time_stack.in_layers.0", "temporal_res_block.norm1"), ("time_stack.in_layers.2", "temporal_res_block.conv1"),
+    ("time_stack.out_layers.0", "temporal_res_block.norm2"), ("time_stack.out_layers.3", "temporal_res_block.conv2"),
+    ("mix_factor", "time_mixer.mix_factor"))
+_VAE_ATTN_MAP = (("norm", "group_norm"), ("q", "to_q"), ("k", "to_k"), ("v", "to_v"), ("proj_out", "to_out.0"))
+
+
+def _vae_prefix_map(plan, n_levels: int, side: str) -> Dict[str, str]:
+    """SGM module prefix -> diffusers module prefix for one side ("encoder" or "decoder") of the VAE."""
+    m = {"conv_in": "conv_in", "mid.block_1": "mid_block.resnets.0", "mid.attn_1": "mid_block.attentions.0",
+         "mid.block_2": "mid_block.resnets.1", "norm_out": "conv_norm_out", "conv_out": "conv_out"}
+    for kind, p, _, _ in plan:
+        parts = p.split(".")
+        if parts[0] == "down":                       # encoder: down_blocks in SGM order
+            i = int(parts[1])
+            m[p] = (f"down_blocks.{i}.resnets.{parts[3]}" if kind == "res" else f"down_blocks.{i}.downsamplers.0")
+        elif parts[0] == "up":                       # decoder: up_blocks.0 is the deepest level, up.{n-1}
+            i = n_levels - 1 - int(parts[1])
+            m[p] = (f"up_blocks.{i}.resnets.{parts[3]}" if kind == "res" else f"up_blocks.{i}.upsamplers.0")
+    if side == "encoder":
+        m["quant_conv"] = "quant_conv"
+    else:
+        m["conv_out.time_mix_conv"] = "time_conv_out"
+    return m
+
+
+def _sgm_to_diffusers_vae_keys(shapes: Dict[str, tuple], plan, n_levels: int, side: str) -> Dict[str, str]:
+    kinds = {p: kind for kind, p, _, _ in plan}
+    prefix = _vae_prefix_map(plan, n_levels, side)
+    out: Dict[str, str] = {}
+    for key in shapes:
+        best = max((p for p in prefix if key.startswith(p + ".")), key=len)
+        rest = key[len(best) + 1:]
+        table = ((_VAE_VIDEO_RES_MAP if side == "decoder" else _VAE_RES_MAP) if kinds.get(best) == "res"
+                 else _VAE_ATTN_MAP if kinds.get(best) == "attn" else ())
+        for a, b in table:
+            if rest == a or rest.startswith(a + "."):
+                rest = b + rest[len(a):]
+                break
+        d = prefix[best] + "." + rest
+        out[key] = d if best == "quant_conv" else f"{side}.{d}"
+    return out
+
+
+def sgm_to_diffusers_vae_encoder_keys(cfg: VaeConfig) -> Dict[str, str]:
+    """vae_encoder_param_shapes key -> key of diffusers' `AutoencoderKLTemporalDecoder.state_dict()`."""
+    return _sgm_to_diffusers_vae_keys(vae_encoder_param_shapes(cfg), vae_encoder_plan(cfg), len(cfg.ch_mult), "encoder")
+
+
+def sgm_to_diffusers_vae_decoder_keys(cfg: VaeConfig) -> Dict[str, str]:
+    """vae_decoder_param_shapes key -> key of diffusers' `AutoencoderKLTemporalDecoder.state_dict()`."""
+    return _sgm_to_diffusers_vae_keys(vae_decoder_param_shapes(cfg), vae_decoder_plan(cfg), len(cfg.ch_mult), "decoder")
+
+
+def from_diffusers_svd_vae_state_dict(sd: Dict[str, "torch.Tensor"], cfg: VaeConfig):
+    """State dict of diffusers' `AutoencoderKLTemporalDecoder` (`svd_pipeline.vae`) -> (encoder, decoder) state dicts
+    in the SGM grammar that B200VaeEncoder (`encoder.*` + `quant_conv.*`) and B200VaeDecoder (`decoder.*`) read.
+
+    The correspondence, restated from diffusers 0.30.2's published source (diffusers is not a dependency: parity is
+    unpinned, as for sgm_to_diffusers_svd_keys; a wrong name fails at load time as a missing key, never silently):
+      down_blocks.i / up_blocks.i    down.i / up.{n-1-i}: the decoder's up_blocks run deepest level first
+      resnets.j.spatial_res_block.*  block.j.*  (conv_shortcut -> nin_shortcut)
+      resnets.j.temporal_res_block   block.j.time_stack  (norm1 / conv1 / norm2 / conv2 -> in_layers.0 / .2,
+                                     out_layers.0 / .3)
+      resnets.j.time_mixer.mix_factor  block.j.mix_factor, unchanged: diffusers' AlphaBlender(merge_strategy="learned",
+                                     switch_spatial_to_temporal_mix=True) takes a = 1 - sigmoid(m) and returns
+                                     a * x_spatial + (1 - a) * x_temporal = (1 - sigmoid(m)) x_s + sigmoid(m) x_t, which
+                                     is SGM VideoResBlock's sigmoid(m) x_t + (1 - sigmoid(m)) x_s for the same m
+      mid_block.attentions.0         mid.attn_1: group_norm -> norm, to_q/k/v -> q/k/v, to_out.0 -> proj_out; the
+                                     diffusers Linear [C, C] is the SGM 1x1 conv [C, C, 1, 1] (a reshape only)
+      conv_norm_out                  norm_out
+      time_conv_out                  conv_out.time_mix_conv
+      downsamplers.0 / upsamplers.0  downsample / upsample
+    Missing keys, keys left over and shape mismatches other than the attention reshape raise."""
+    out = []
+    used = set()
+    for m, shapes in ((sgm_to_diffusers_vae_encoder_keys(cfg), vae_encoder_param_shapes(cfg)),
+                      (sgm_to_diffusers_vae_decoder_keys(cfg), vae_decoder_param_shapes(cfg))):
+        missing = [d for d in m.values() if d not in sd]
+        if missing:
+            raise KeyError(f"{len(missing)} keys missing in the diffusers VAE state dict, e.g. {missing[:4]}")
+        part = {}
+        for k, d in m.items():
+            t = sd[d]
+            if t.dim() == 2 and len(shapes[k]) == 4:       # attention Linear -> 1x1 conv
+                t = t.reshape(shapes[k])
+            part[k] = t
+        _check_shapes(part, shapes, "VAE")
+        used.update(m.values())
+        out.append(part)
+    extra = sorted(k for k in sd if k not in used)
+    if extra:
+        raise KeyError(f"{len(extra)} VAE keys without an SGM counterpart, e.g. {extra[:4]}")
+    return out[0], out[1]

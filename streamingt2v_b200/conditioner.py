@@ -22,7 +22,7 @@ import torch
 
 from . import dist_utils, ops, packing
 from ._lib import ACT_GELU
-from .arch import ClipVisionConfig
+from .arch import ClipVisionConfig, VaeConfig
 
 SD = Dict[str, torch.Tensor]
 CLIP_SIZE = 224
@@ -120,13 +120,19 @@ class B200SVDConditioner:
     cond_frames = image + cond_aug * U[0, 1) noise (streaming_svd.py:174; `torch.rand_like`, uniform).  With
     `generator` the noise is `torch.rand(image.shape, generator=generator, device=generator.device)`; without one it
     comes from torch's global generator, as in the reference.  Under torch.distributed with more than one rank, rank
-    0's noise is broadcast so that every rank conditions on the same frames."""
+    0's noise is broadcast so that every rank conditions on the same frames.
+
+    `noise="gaussian"` draws N(0, 1) noise instead (`torch.randn`, same generator rules): the conditioning of diffusers'
+    StableVideoDiffusionPipeline, which makes the first chunk of a request (see `from_diffusers_svd`)."""
 
     def __init__(self, clip: B200ClipImageEncoder, vae_encoder, *, generator: Optional[torch.Generator] = None,
-                 fps_id: int = 6, motion_bucket_id: int = 127, cond_aug: float = 0.02):
+                 fps_id: int = 6, motion_bucket_id: int = 127, cond_aug: float = 0.02, noise: str = "uniform"):
+        if noise not in ("uniform", "gaussian"):
+            raise ValueError(f"noise must be 'uniform' or 'gaussian', got {noise!r}")
         self.clip, self.vae_encoder = clip, vae_encoder
         self.generator = generator
         self.fps_id, self.motion_bucket_id, self.cond_aug = fps_id, motion_bucket_id, float(cond_aug)
+        self.noise = noise
         self.dev = clip.dev
 
     @classmethod
@@ -134,7 +140,6 @@ class B200SVDConditioner:
         """Build from the reference's instantiated `GeneralConditioner` (config.yaml:159-218): the image tower from
         `embedders[0].open_clip.model.visual.state_dict()`, the VAE encoder from `embedders[3].encoder.encoder.*` and
         `embedders[3].encoder.quant_conv.*`."""
-        from .arch import VaeConfig
         from .vae import B200VaeEncoder
         sd_v = conditioner.embedders[0].open_clip.model.visual.state_dict()
         layers = sum(1 for k in sd_v if k.startswith("transformer.resblocks.") and k.endswith(".attn.in_proj_weight"))
@@ -154,26 +159,69 @@ class B200SVDConditioner:
                          z_channels=sd_e["quant_conv.weight"].shape[0] // 2)
         return cls(B200ClipImageEncoder(ccfg, sd_v, device), B200VaeEncoder(vcfg, sd_e, device), **kw)
 
-    def _noise(self, image: torch.Tensor) -> torch.Tensor:
-        g = self.generator
-        if g is not None:
-            noise = torch.rand(image.shape, generator=g, device=g.device)
+    @classmethod
+    def from_diffusers_svd(cls, pipeline, device="cuda:0", **kw):
+        """The conditioning of diffusers' `StableVideoDiffusionPipeline` (`svd_pipeline`, streaming_svd.py:62,390) on
+        this class, built from `pipeline.image_encoder` (transformers CLIPVisionModelWithProjection, renamed by
+        arch.from_hf_clip_vision_state_dict) and `pipeline.vae` (AutoencoderKLTemporalDecoder, encoder + quant_conv
+        renamed by arch.from_diffusers_svd_vae_state_dict), with Gaussian noise.  The pipeline computes the same
+        function as this class (restated from diffusers 0.30.2's published source; diffusers is not a dependency, so
+        parity is unpinned):
+          * CLIP runs on the clean image through `_resize_with_antialiasing(image * 2 - 1, (224, 224))`, then
+            `(x + 1) / 2` and the CLIP normalisation: kornia's antialias resize that `clip_preprocess` restates.  Its
+            taps are kornia's wherever kornia blurs; where kornia skips the blur (no axis downscaled, or a 224 x 224
+            input) diffusers blurs with sigma 0.001, taps [0, 1, 0] in fp32, and a same-size align_corners bicubic
+            resize samples the grid points exactly: the same output as no blur;
+          * the VAE encodes `(image * 2 - 1) + noise_aug_strength * randn`, noise drawn before the latents, and the
+            latent is the posterior mode, unscaled;
+          * the negative image embedding and latent are zero;
+          * `added_time_ids = [fps - 1, motion_bucket_id, noise_aug_strength]` go through
+            `Timesteps(256, flip_sin_to_cos=True, downscale_freq_shift=0)`: [cos | sin] per id, the `vector` built here
+            with fps_id = fps - 1 and cond_aug = noise_aug_strength, the same for both guidance halves."""
+        from .arch import clip_vision_config_from_hf, from_diffusers_svd_vae_state_dict, from_hf_clip_vision_state_dict
+        from .vae import B200VaeEncoder
+        enc = pipeline.image_encoder
+        ccfg = clip_vision_config_from_hf(enc.config)
+        sd_v = from_hf_clip_vision_state_dict(enc.state_dict(), enc.config)
+        vcfg = vae_config_from_diffusers(pipeline.vae.config)
+        sd_e, _ = from_diffusers_svd_vae_state_dict(pipeline.vae.state_dict(), vcfg)
+        kw.setdefault("noise", "gaussian")
+        return cls(B200ClipImageEncoder(ccfg, sd_v, device), B200VaeEncoder(vcfg, sd_e, device), **kw)
+
+    def _noise(self, image: torch.Tensor, generator: Optional[torch.Generator]) -> torch.Tensor:
+        draw, draw_like = (torch.rand, torch.rand_like) if self.noise == "uniform" else (torch.randn, torch.randn_like)
+        if generator is not None:
+            noise = draw(image.shape, generator=generator, device=generator.device)
         else:
-            noise = torch.rand_like(image)
+            noise = draw_like(image)
         noise = noise.to(self.dev, torch.float32)
         return dist_utils.broadcast_from_rank0(noise)
 
     @torch.no_grad()
     def __call__(self, frame: torch.Tensor, num_frames: int):
-        T = int(num_frames)
+        return self.condition(frame, num_frames, fps_id=self.fps_id, motion_bucket_id=self.motion_bucket_id,
+                              cond_aug=self.cond_aug, generator=self.generator)
+
+    @torch.no_grad()
+    def condition(self, frame: torch.Tensor, num_frames: int, *, fps_id: int, motion_bucket_id: int, cond_aug: float,
+                  generator: Optional[torch.Generator]):
+        """`__call__` with the micro-conditioning values and the noise generator of one request."""
+        T, cond_aug = int(num_frames), float(cond_aug)
         image = frame[None].to(self.dev, torch.float32).contiguous()                    # [1, 3, H, W]
-        cond_frames = image + self.cond_aug * self._noise(image)
+        cond_frames = image + cond_aug * self._noise(image, generator)
         crossattn = self.clip.encode(image)[:, None, :]                                # [1, 1, 1024]
         concat = self.vae_encoder.encode(cond_frames)                                   # [1, 4, H/8, W/8], scale 1.0
-        t = torch.tensor([float(self.fps_id)] * T + [float(self.motion_bucket_id)] * T + [self.cond_aug] * T,
+        t = torch.tensor([float(fps_id)] * T + [float(motion_bucket_id)] * T + [cond_aug] * T,
                          dtype=torch.float32, device=self.dev)
         emb = ops.timestep_embed(t, 256)                                                # [(3 T), 256] bf16
         vector = emb.float().view(3, T, 256).transpose(0, 1).reshape(T, 768)           # [fps | motion | cond_aug]
         c = {"crossattn": crossattn, "concat": concat, "vector": vector}
         uc = {"crossattn": torch.zeros_like(crossattn), "concat": torch.zeros_like(concat), "vector": vector.clone()}
         return c, uc
+
+
+def vae_config_from_diffusers(config) -> VaeConfig:
+    """VaeConfig of an `AutoencoderKLTemporalDecoder.config` (block_out_channels, layers_per_block, latent_channels)."""
+    boc = tuple(config.block_out_channels)
+    return VaeConfig(ch=boc[0], ch_mult=tuple(c // boc[0] for c in boc), num_res_blocks=int(config.layers_per_block),
+                     z_channels=int(config.latent_channels), out_ch=int(getattr(config, "out_channels", 3)))

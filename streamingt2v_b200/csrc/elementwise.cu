@@ -390,6 +390,20 @@ __global__ void frames_to_uint8_kernel(const float* __restrict__ x, uint8_t* __r
   }
 }
 
+// The uint8 image round trip of the first chunk, in place of diffusers' postprocess_video(output_type="pil") followed by
+// torchvision's ToTensor() and `* 2.0 - 1` (streaming_svd.py:390-393).  Each step is one fp32 operation rounded to
+// nearest, in the reference's order; the explicit _rn intrinsics keep nvcc from contracting them into FMAs.
+// 255 is not a power of two, so neither `* 255` nor `/ 255` is exact and the order matters.
+__global__ void frames_quantize_kernel(const float* x, float* out, int64_t n) {  // out may alias x
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  float v = __fadd_rn(__fdiv_rn(x[i], 2.0f), 0.5f);   // x / 2 + 0.5
+  v = fminf(fmaxf(v, 0.0f), 1.0f);                    // .clamp(0, 1)
+  v = rintf(__fmul_rn(v, 255.0f));                    // (v * 255).round(): numpy rounds half to even, as rintf does
+  v = __fdiv_rn(v, 255.0f);                           // ToTensor: uint8 -> float / 255
+  out[i] = __fsub_rn(__fmul_rn(v, 2.0f), 1.0f);       // * 2.0 - 1
+}
+
 }  // namespace b200
 
 extern "C" {
@@ -406,6 +420,18 @@ int b200svd_frames_to_uint8(const float* x, void* out, int64_t n, int c, int64_t
   frames_to_uint8_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
       x, reinterpret_cast<uint8_t*>(out), n, c, hw, vmin, vmax);
   B200_CHECK_LAUNCH("frames_to_uint8");
+  return 0;
+}
+
+int b200svd_frames_quantize(const float* x, float* out, int64_t n, void* stream) {
+  using namespace b200;
+  if (n < 0) {
+    set_error("frames_quantize: negative element count");
+    return 1;
+  }
+  if (n == 0) return 0;
+  frames_quantize_kernel<<<(unsigned)((n + 255) / 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(x, out, n);
+  B200_CHECK_LAUNCH("frames_quantize");
   return 0;
 }
 

@@ -667,6 +667,17 @@ def frames_to_uint8(x, vmin=0.0, vmax=255.0):
     return out
 
 
+def frames_quantize(x, out=None):
+    """fp32 frames in [-1, 1] -> fp32 on the 1/127.5 grid: the 8-bit image round trip of the first chunk
+    (diffusers' postprocess_video to PIL, ToTensor(), `* 2.0 - 1`; streaming_svd.py:390-393), rounding half to even."""
+    assert x.dtype == torch.float32 and x.is_contiguous()
+    if out is None:
+        out = torch.empty_like(x)
+    assert out.dtype == torch.float32 and out.is_contiguous() and out.shape == x.shape
+    _call("b200svd_frames_quantize", _ptr(x), _ptr(out), x.numel(), _stream(), nbytes=8.0 * x.numel())
+    return out
+
+
 def attention_single_head(q, k, v, n, s):
     """softmax(q k^T / sqrt(C)) v per frame, one head of width C (VAE AttnBlock).  q, k, v: contiguous [(n s), C] bf16.
     Built from the tensor-core GEMM (scores in fp32), a row-softmax kernel and a transpose."""

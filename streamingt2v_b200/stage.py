@@ -20,6 +20,7 @@ from __future__ import annotations
 import math
 from typing import Callable, List, Optional, Sequence, Union
 
+import numpy as np
 import torch
 
 from . import dist_utils
@@ -27,12 +28,23 @@ from . import dist_utils
 SCALE_FACTOR = 0.18215      # config.yaml scale_factor (diff_trainer_params.scale_factor)
 MAX_DECODE_CHUNK = 8        # streaming_svd.py:127 (4 with use_memopt)
 SPATIAL_COMPRESSION = 8     # streaming_svd.py:157
+IMAGE_HEIGHT, IMAGE_WIDTH = 576, 1024   # streaming_svd.py:384-385
 
 
 def convert_range(video: torch.Tensor, output_range: Sequence[float], input_range: Sequence[float]) -> torch.Tensor:
     """utils/result_processor.py:4-14 with an explicit input range."""
     video = (video - input_range[0]) / (input_range[1] - input_range[0])
     return video * (output_range[1] - output_range[0]) + output_range[0]
+
+
+def resize_and_keep(image):
+    """utils/inference_utils.py:37-42: PIL resize to height 576, width scaled by the same factor (truncated), with
+    Pillow's default filter.  `image` is a PIL image or a uint8 [H, W, 3] array; returns a PIL image."""
+    from PIL import Image
+    if not isinstance(image, Image.Image):
+        image = Image.fromarray(np.asarray(image, dtype=np.uint8))
+    hpercent = IMAGE_HEIGHT / float(image.size[1])
+    return image.resize((int(float(image.size[0]) * float(hpercent)), IMAGE_HEIGHT))
 
 
 def _to_fchw(video: torch.Tensor) -> torch.Tensor:
@@ -140,6 +152,18 @@ class B200StreamingSVDStage:
             chunks.append(result[self.num_conditional_frames:])         # :347 keep all but the conditioning frames
         chunks = [convert_range(ch.to(torch.float32), [0, 255], [-1, 1]) for ch in chunks]
         return torch.cat([ch.to(chunks[0].device) for ch in chunks], dim=0)
+
+    # -- streaming_svd.py:359-399 ----------------------------------------------------------------------------------
+    def image_to_video(self, image, n_autoregressive_generations: int, first_chunk: Callable,
+                       generator: Optional[torch.Generator] = None) -> torch.Tensor:
+        """image (PIL image or uint8 [H, W, 3]) -> the whole video [F_total, C, H, W] in [0, 255].  The image is resized
+        to height 576 on the host (one image per request) and must then be 1024 x 576; `first_chunk` (normally a
+        `first_chunk.B200SVDImageToVideo`) makes the first chunk from it with the same `generator`, and
+        `autoregressive_generation` continues from there."""
+        img = resize_and_keep(image)
+        assert img.width == IMAGE_WIDTH and img.height == IMAGE_HEIGHT, f"image resized to {img.size}, need 1024x576"
+        video_chunks = first_chunk(np.asarray(img.convert("RGB")), generator=generator)
+        return self.autoregressive_generation(video_chunks.to(self.device), n_autoregressive_generations, generator)
 
     def to_uint8_frames(self, video: torch.Tensor) -> torch.Tensor:
         """[F,C,H,W] float in [0, 255] -> uint8 [F,H,W,C] ON THE DEVICE: the array the reference's IImage container
