@@ -182,13 +182,22 @@ int b200svd_pixel_attn(const void* q, int64_t ldq, const void* k, int64_t ldk, c
  * video_attention.py:59-102, controlnet.py:113-118).
  * x: [n][p][c] rows (stride ldx).  sums: n*32*2 doubles (sum, sum of squares).  The reduction is deterministic
  * (fixed order, no floating-point atomics): scratch holds per-chunk partials (b200svd_gn_scratch_doubles doubles),
- * counters is n int32 zero-initialised once by the caller (left zero by every call). */
+ * counters is n int32 zero-initialised once by the caller (left zero by every call).
+ * Every GroupNorm entry point returns an error, before any launch, unless 32 <= c <= 8192 with c % 32 == 0,
+ * 0 <= n <= 65535 and 0 <= p <= INT_MAX (b200svd_gn_scratch_doubles returns -1 instead); gn_stats and gn_apply
+ * further need leading dims that are multiples of 8 and 16-byte aligned x (and y).  n = 0 or p = 0 launches nothing,
+ * writes nothing and returns 0 (scratch: 0 doubles).  gn_apply runs one thread per 8 channels in one block, so it also
+ * returns an error when c / 8 exceeds the threads per block its register use allows (c <= 7168 on sm_90a);
+ * gn_stats takes every c up to 8192. */
 int64_t b200svd_gn_scratch_doubles(int64_t n, int64_t p, int c);
 int b200svd_gn_stats(const void* x, int64_t ldx, int64_t n, int64_t p, int c, void* sums, void* scratch,
                      void* counters, void* stream);
 int b200svd_gn_apply(const void* x, int64_t ldx, void* y, int64_t ldy, int64_t n, int64_t p, int c, const void* sums,
                      const float* gamma, const float* beta, float eps, int apply_silu, void* stream);
-/* y = LN(x [+ fvec[row / rows_per_frame]]) ; if xsum != NULL also writes xsum = bf16(x + fvec). */
+/* y = LN(x [+ fvec[row / rows_per_frame]]) ; if xsum != NULL also writes xsum = bf16(x + fvec).
+ * Errors, before any launch: c not a multiple of 8 in [0, 2048]; ldx, ldy (and ldxs with xsum) not multiples of 8;
+ * xsum without fvec; x, y or xsum not 16-byte aligned.  gamma / beta / fvec may have any 4-byte alignment (a scalar
+ * kernel takes over).  rows = 0 or c = 0 launches nothing and returns 0. */
 int b200svd_layernorm(const void* x, int64_t ldx, void* y, int64_t ldy, int64_t rows, int c, const float* gamma,
                       const float* beta, float eps, const float* fvec, int64_t ldf, int rows_per_frame, void* xsum,
                       int64_t ldxs, int apply_silu, void* stream);
@@ -200,7 +209,10 @@ int b200svd_layernorm(const void* x, int64_t ldx, void* y, int64_t ldy, int64_t 
  * upsample2x: Upsample nearest (openaimodel.py:138-155).  timestep_embed: util.py:207-231.
  * add_silu: out = bf16(silu(a + b)) for emb = time_embed + label_emb followed by emb_layers' SiLU
  *   (video_model.py:561-567, openaimodel.py:282-288).  add_rows: ControlNet Merger addition (controlnet.py:23-48).
- * apm_mix: BasicTransformerBlockWithAPM context mix (attention.py:612-620). */
+ * apm_mix: BasicTransformerBlockWithAPM context mix (attention.py:612-620).
+ * Every glue entry point below, softmax_rows and transpose included, launches nothing and returns 0 when its output
+ * has no elements.  Before any launch they return an error for: upsample2x, copy2d, add_rows operands not 16-byte
+ * aligned; add_rows src_rows < 1; softmax_rows `in` not 16-byte or `out` not 8-byte aligned. */
 int b200svd_nchw_to_nhwc(const float* src, int64_t src_frame_stride, int n, int c_src, int64_t hw, void* dst,
                          int64_t ldd, int c_off, void* stream);
 int b200svd_nhwc_to_nchw(const void* src, int src_is_fp32, int64_t lds, int n, int c, int64_t hw, float* dst,

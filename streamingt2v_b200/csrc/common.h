@@ -27,6 +27,9 @@ int encode_tmap_bf16_sw32(CUtensorMap* out, const void* gptr, int rank, const ui
 
 int sm_count();
 
+// true if p is a multiple of `bytes` (a power of two): the base a kernel's 8- or 16-byte vector accesses need
+inline bool aligned(const void* p, uintptr_t bytes) { return (reinterpret_cast<uintptr_t>(p) & (bytes - 1)) == 0; }
+
 // Launch-attribute caches (cudaFuncSetAttribute results, occupancy queries) are kept PER DEVICE: function attributes
 // belong to a device's context, and one process may drive several GPUs (the reference does not, but the caches must not
 // silently assume it).  Index of the calling thread's current device, folded into [0, B200_MAX_DEVICES).

@@ -187,6 +187,7 @@ extern "C" {
 int b200svd_nchw_to_nhwc(const float* src, int64_t src_frame_stride, int n, int c_src, int64_t hw, void* dst,
                          int64_t ldd, int c_off, void* stream) {
   using namespace b200;
+  if (n <= 0 || hw <= 0) return 0;
   const int64_t total = (int64_t)n * hw;
   nchw_to_nhwc_kernel<<<blocks_for(total, 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
       src, src_frame_stride, c_src, hw, reinterpret_cast<__nv_bfloat16*>(dst), ldd, c_off, total);
@@ -197,6 +198,7 @@ int b200svd_nchw_to_nhwc(const float* src, int64_t src_frame_stride, int n, int 
 int b200svd_nhwc_to_nchw(const void* src, int src_is_fp32, int64_t lds, int n, int c, int64_t hw, float* dst,
                          void* stream) {
   using namespace b200;
+  if (n <= 0 || c <= 0 || hw <= 0) return 0;
   const int64_t total = (int64_t)n * c * hw;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   if (src_is_fp32)
@@ -215,6 +217,11 @@ int b200svd_upsample2x(const void* x, void* y, int n, int h, int w, int c, void*
     set_error("upsample2x: channels must be a multiple of 8");
     return 1;
   }
+  if (n <= 0 || h <= 0 || w <= 0 || c <= 0) return 0;
+  if (!aligned(x, 16) || !aligned(y, 16)) {  // one 16-byte vector per thread
+    set_error("upsample2x: x and y must be 16-byte aligned");
+    return 1;
+  }
   const int vecs = c / 8;
   const int64_t total = (int64_t)n * 2 * h * 2 * w * vecs;
   upsample2x_kernel<<<blocks_for(total, 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
@@ -229,6 +236,7 @@ int b200svd_timestep_embed(const float* t, int n, int dim, float max_period, voi
     set_error("timestep_embed: odd dim unsupported");
     return 1;
   }
+  if (n <= 0 || dim <= 0) return 0;
   const int total = n * (dim / 2);
   timestep_embed_kernel<<<blocks_for(total, 128), 128, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
       t, n, dim, max_period, reinterpret_cast<__nv_bfloat16*>(out), ldo);
@@ -238,6 +246,7 @@ int b200svd_timestep_embed(const float* t, int n, int dim, float max_period, voi
 
 int b200svd_add_silu(const float* a, const float* b, void* out, int64_t total, int apply_silu, void* stream) {
   using namespace b200;
+  if (total <= 0) return 0;
   add_silu_kernel<<<blocks_for(total, 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
       a, b, reinterpret_cast<__nv_bfloat16*>(out), total, apply_silu);
   B200_CHECK_LAUNCH("add_silu");
@@ -248,6 +257,11 @@ int b200svd_copy2d(const void* src, int64_t lds, void* dst, int64_t ldd, int64_t
   using namespace b200;
   if (cols % 8 || lds % 8 || ldd % 8) {
     set_error("copy2d: cols and leading dims must be multiples of 8");
+    return 1;
+  }
+  if (rows <= 0 || cols <= 0) return 0;
+  if (!aligned(src, 16) || !aligned(dst, 16)) {  // 16-byte vectors
+    set_error("copy2d: src and dst must be 16-byte aligned");
     return 1;
   }
   const int vecs = cols / 8;
@@ -263,6 +277,15 @@ int b200svd_add_rows(void* dst, int64_t ldd, const void* src, int64_t lds, int64
   using namespace b200;
   if (cols % 8 || lds % 8 || ldd % 8) {
     set_error("add_rows: cols and leading dims must be multiples of 8");
+    return 1;
+  }
+  if (src_rows < 1) {  // dst row r adds src row r % src_rows
+    set_error("add_rows: src_rows must be >= 1 (got %lld)", (long long)src_rows);
+    return 1;
+  }
+  if (rows <= 0 || cols <= 0) return 0;
+  if (!aligned(dst, 16) || !aligned(src, 16)) {  // 16-byte vectors
+    set_error("add_rows: dst and src must be 16-byte aligned");
     return 1;
   }
   const int vecs = cols / 8;
@@ -281,6 +304,7 @@ int b200svd_apm_mix(const float* ctx, int n, int l, int d, const float* w, const
     set_error("apm_mix: D too large");
     return 1;
   }
+  if (n <= 0 || d <= 0) return 0;
   apm_mix_kernel<<<n, 256, d * sizeof(float), reinterpret_cast<cudaStream_t>(stream)>>>(
       ctx, l, d, w, wb, ln_g, ln_b, alpha, reinterpret_cast<__nv_bfloat16*>(out));
   B200_CHECK_LAUNCH("apm_mix");
@@ -464,6 +488,11 @@ int b200svd_softmax_rows(const float* in, int64_t lds, void* out, int64_t ldo, i
     set_error("softmax_rows: cols and leading dims must be multiples of 4");
     return 1;
   }
+  if (rows <= 0 || cols <= 0) return 0;
+  if (!aligned(in, 16) || !aligned(out, 8)) {  // float4 loads, 4 x bf16 (8-byte) stores
+    set_error("softmax_rows: in must be 16-byte and out 8-byte aligned");
+    return 1;
+  }
   softmax_rows_kernel<<<(unsigned)rows, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
       in, lds, reinterpret_cast<__nv_bfloat16*>(out), ldo, cols);
   B200_CHECK_LAUNCH("softmax_rows");
@@ -472,6 +501,7 @@ int b200svd_softmax_rows(const float* in, int64_t lds, void* out, int64_t ldo, i
 
 int b200svd_transpose(const void* in, int64_t ldi, void* out, int64_t ldo, int rows, int cols, void* stream) {
   using namespace b200;
+  if (rows <= 0 || cols <= 0) return 0;
   dim3 grid((cols + 31) / 32, (rows + 31) / 32), block(32, 8);
   transpose_kernel<<<grid, block, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
       reinterpret_cast<const __nv_bfloat16*>(in), ldi, reinterpret_cast<__nv_bfloat16*>(out), ldo, rows, cols);

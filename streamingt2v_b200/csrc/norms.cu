@@ -4,6 +4,7 @@
 // Normalize (attention.py:132-135, eps 1e-6), the CAM joint (C/32,F,H,W) GroupNorm (code/models/cam/conditioning.py:57-59),
 // nn.LayerNorm (attention.py:528-530, video_attention.py:59,87,101-102; controlnet.py:113-118).
 #include <cuda_bf16.h>
+#include <limits.h>
 
 #include "../../include/b200svd.h"
 #include "common.h"
@@ -530,6 +531,20 @@ static int gn_geometry(int C, int64_t n, int P, int* threads, int* rows_per_chun
   return 0;
 }
 
+// Shapes every GroupNorm entry point accepts: 32 <= c <= 8192 in whole groups of channels (gn_geometry), p within the
+// kernels' int row index, n within gridDim.y.  n = 0 or p = 0 is valid and launches nothing.
+static int gn_check_shape(const char* who, int64_t n, int64_t p, int c) {
+  if (c < 32 || c > 8192 || c % 32 != 0) {
+    set_error("%s: unsupported channel count %d (need a multiple of 32, 32 <= c <= 8192)", who, c);
+    return 1;
+  }
+  if (n < 0 || n > 65535 || p < 0 || p > INT_MAX) {
+    set_error("%s: need 0 <= n <= 65535 and 0 <= p <= %d (n %lld, p %lld)", who, INT_MAX, (long long)n, (long long)p);
+    return 1;
+  }
+  return 0;
+}
+
 }  // namespace b200
 
 extern "C" {
@@ -538,6 +553,8 @@ extern "C" {
 // zero-initialised once by the caller (the kernel leaves them zero).
 int64_t b200svd_gn_scratch_doubles(int64_t n, int64_t p, int c) {
   using namespace b200;
+  if (gn_check_shape("gn_scratch_doubles", n, p, c)) return -1;
+  if (n == 0 || p == 0) return 0;
   int threads, rpc, chunks;
   if (gn_geometry(c, n, (int)p, &threads, &rpc, &chunks)) return -1;
   return n * (int64_t)chunks * 64;
@@ -546,9 +563,9 @@ int64_t b200svd_gn_scratch_doubles(int64_t n, int64_t p, int c) {
 int b200svd_gn_stats_partials(const float* gn_part, const int32_t* gn_slot_sample, int64_t n_slots, int64_t gn_ld,
                               int c, int64_t n, void* sums, void* scratch, void* counters, void* stream) {
   using namespace b200;
-  if (c % 32 != 0 || c < 256 || c > 8192 || gn_ld < c || n_slots < 1 || n < 1) {
-    set_error("gn_stats_partials: need 256 <= c <= 8192, c %% 32 == 0, gn_ld >= c (c %d, ld %lld, slots %lld)", c,
-              (long long)gn_ld, (long long)n_slots);
+  if (c % 32 != 0 || c < 256 || c > 8192 || gn_ld < c || n_slots < 1 || n < 1 || n > 65535) {
+    set_error("gn_stats_partials: need 256 <= c <= 8192, c %% 32 == 0, gn_ld >= c, n_slots >= 1, 1 <= n <= 65535 "
+              "(c %d, ld %lld, slots %lld, n %lld)", c, (long long)gn_ld, (long long)n_slots, (long long)n);
     return 1;
   }
   const int64_t chunks = (n_slots + GNP_SLOTS - 1) / GNP_SLOTS;
@@ -571,13 +588,19 @@ int b200svd_gn_stats_partials(const float* gn_part, const int32_t* gn_slot_sampl
 int b200svd_gn_stats(const void* x, int64_t ldx, int64_t n, int64_t p, int c, void* sums, void* scratch,
                      void* counters, void* stream) {
   using namespace b200;
-  int threads, rpc, chunks;
-  if (gn_geometry(c, n, (int)p, &threads, &rpc, &chunks)) {
-    set_error("gn_stats: unsupported channel count %d (need multiple of 32, <= 8192)", c);
-    return 1;
-  }
+  if (gn_check_shape("gn_stats", n, p, c)) return 1;
   if (ldx % 8 != 0) {
     set_error("gn_stats: ldx must be a multiple of 8");
+    return 1;
+  }
+  if (n == 0 || p == 0) return 0;
+  if (!aligned(x, 16)) {  // 16-byte (8-channel) loads
+    set_error("gn_stats: x must be 16-byte aligned");
+    return 1;
+  }
+  int threads, rpc, chunks;
+  if (gn_geometry(c, n, (int)p, &threads, &rpc, &chunks)) {
+    set_error("gn_stats: unsupported channel count %d", c);
     return 1;
   }
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
@@ -601,13 +624,34 @@ int b200svd_gn_stats(const void* x, int64_t ldx, int64_t n, int64_t p, int c, vo
 int b200svd_gn_apply(const void* x, int64_t ldx, void* y, int64_t ldy, int64_t n, int64_t p, int c, const void* sums,
                      const float* gamma, const float* beta, float eps, int apply_silu, void* stream) {
   using namespace b200;
+  if (gn_check_shape("gn_apply", n, p, c)) return 1;
+  if (ldx % 8 != 0 || ldy % 8 != 0) {
+    set_error("gn_apply: leading dims must be multiples of 8");
+    return 1;
+  }
+  if (n == 0 || p == 0) return 0;
+  if (!aligned(x, 16) || !aligned(y, 16)) {  // 16-byte (8-channel) loads and stores
+    set_error("gn_apply: x and y must be 16-byte aligned");
+    return 1;
+  }
   int threads, rpc, chunks;
   if (gn_geometry(c, n, (int)p, &threads, &rpc, &chunks)) {
     set_error("gn_apply: unsupported channel count %d", c);
     return 1;
   }
-  if (ldx % 8 != 0 || ldy % 8 != 0) {
-    set_error("gn_apply: leading dims must be multiples of 8");
+  // one thread per 8-channel column: past c = 2048 a block has c / 8 threads, and the kernel's register use caps the
+  // block below 1024 threads (at 66 registers, 896: c <= 7168)
+  static int max_threads_dev[B200_MAX_DEVICES] = {};
+  int& max_threads = max_threads_dev[dev_slot()];
+  if (max_threads == 0) {
+    cudaFuncAttributes fa;
+    cudaError_t e = cudaFuncGetAttributes(&fa, gn_apply_kernel);
+    if (e != cudaSuccess) return cuda_fail(e, "cudaFuncGetAttributes(gn_apply)");
+    max_threads = fa.maxThreadsPerBlock;
+  }
+  if (threads > max_threads) {
+    set_error("gn_apply: c = %d needs %d threads per block, the kernel launches at most %d (c <= %d)", c, threads,
+              max_threads, max_threads / 4 * 32);
     return 1;
   }
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
@@ -623,12 +667,22 @@ int b200svd_layernorm(const void* x, int64_t ldx, void* y, int64_t ldy, int64_t 
                       const float* beta, float eps, const float* fvec, int64_t ldf, int rows_per_frame, void* xsum,
                       int64_t ldxs, int apply_silu, void* stream) {
   using namespace b200;
-  if (c % 8 != 0 || c > 8 * 32 * 8) {
+  if (c < 0 || c % 8 != 0 || c > 8 * 32 * 8) {
     set_error("layernorm: unsupported width %d (multiple of 8, <= 2048)", c);
     return 1;
   }
   if (ldx % 8 != 0 || ldy % 8 != 0 || (xsum && ldxs % 8 != 0)) {
     set_error("layernorm: leading dims must be multiples of 8");
+    return 1;
+  }
+  if (xsum && !fvec) {  // the kernels write xsum = bf16(x + fvec) only while adding fvec
+    set_error("layernorm: xsum needs fvec (xsum = bf16(x + fvec)); pass both or neither");
+    return 1;
+  }
+  if (rows <= 0 || c == 0) return 0;
+  // x, y and xsum move in 16-byte vectors; gamma / beta / fvec fall back to the scalar kernel below when misaligned
+  if (!aligned(x, 16) || !aligned(y, 16) || !aligned(xsum, 16)) {
+    set_error("layernorm: x, y and xsum must be 16-byte aligned");
     return 1;
   }
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);

@@ -503,9 +503,10 @@ def group_norm(x, n, p, gamma, beta, eps, *, silu=False, out=None, sums=None):
               _ptr(scratch), _ptr(counters), _stream(), nbytes=8.0 * gn["n_slots"] * Cc,
               desc=f"stats(partials) n{n} p{p} c{Cc}")
     else:
-        need = _lib.load().b200svd_gn_scratch_doubles(n, p, Cc)
+        lib = _lib.load()
+        need = lib.b200svd_gn_scratch_doubles(n, p, Cc)
         if need < 0:
-            raise _lib.B200Error(f"group_norm: unsupported channel count {Cc}")
+            raise _lib.B200Error(f"group_norm: {lib.b200svd_last_error().decode()}")
         scratch, counters = _gn_scratch(x.device, need, n)
         _call("b200svd_gn_stats", _ptr(x), x.stride(0), n, p, Cc, _ptr(sums), _ptr(scratch), _ptr(counters), _stream(),
               nbytes=2.0 * n * p * Cc, desc=f"stats n{n} p{p} c{Cc}")
@@ -516,6 +517,7 @@ def group_norm(x, n, p, gamma, beta, eps, *, silu=False, out=None, sums=None):
 
 def layer_norm(x, gamma, beta, eps=1e-5, *, fvec=None, rows_per_frame=1, xsum=None, silu=False, out=None):
     assert x.dtype == torch.bfloat16 and x.dim() == 2 and x.stride(1) == 1
+    assert xsum is None or fvec is not None, "layer_norm: xsum = bf16(x + fvec) needs fvec"
     rows, Cc = x.shape
     if out is None:
         out = torch.empty((rows, Cc), dtype=torch.bfloat16, device=x.device)

@@ -2,8 +2,10 @@
 
 The GEMM epilogue stores fp32 column pairs as one 8-byte float2 and loads residual pairs as 4-byte words; the
 attention kernels move 16-byte chunks (cp.async, uint4) or store 4-byte words from a 16-byte aligned base.  A
-misaligned base must come back as an error, never reach a launch.  The pointers below are fake host addresses, so
-these tests only run where no CUDA device is visible: the checks must return before anything touches them."""
+misaligned base must come back as an error, never reach a launch.  The norm and glue kernels move 16-byte vectors
+(softmax_rows stores 8-byte ones).  The same holds for the other argument checks of those entry points, and a call
+with nothing to compute returns 0 without a launch.  The pointers below are fake host addresses, so these tests only
+run where no CUDA device is visible: the checks must return before anything touches them."""
 import ctypes as C
 
 import pytest
@@ -94,3 +96,147 @@ def test_small_attn_routes_on_kv_per_pixel_alone(monkeypatch):
     ops.small_attn(t, t, t, b=1, s=1, heads=1, lq=8, lk=8, kv_per_pixel=True, out=t)
     ops.small_attn(t, t, t[:1], b=1, s=1, heads=1, lq=8, lk=1, kv_per_pixel=False, out=t)
     assert calls == ["b200svd_pixel_attn", "b200svd_small_attn"]
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# norm and glue entry points: 16-byte vector accesses (softmax_rows stores 8-byte groups of four bf16)
+# ---------------------------------------------------------------------------------------------------------------------
+X, Y, Z = BASE, BASE + 0x1000000, BASE + 0x2000000   # three aligned fake operands, far apart
+GAMMA, BETA = BASE + 0x3000000, BASE + 0x3100000
+
+
+def _layernorm(lib, x=X, y=Y, xsum=None, fvec=None, rows=8, c=320):
+    return lib.b200svd_layernorm(x, c, y, c, rows, c, GAMMA, BETA, 1e-5, fvec, c if fvec else 0, 4, xsum,
+                                 c if xsum else 0, 0, None)
+
+
+MISALIGNED = {
+    "gn_stats_x": lambda lib: lib.b200svd_gn_stats(X + 8, 320, 2, 64, 320, Y, Z, Z + 0x100000, None),
+    "gn_apply_x": lambda lib: lib.b200svd_gn_apply(X + 8, 320, Y, 320, 2, 64, 320, Z, GAMMA, BETA, 1e-5, 0, None),
+    "gn_apply_y": lambda lib: lib.b200svd_gn_apply(X, 320, Y + 2, 320, 2, 64, 320, Z, GAMMA, BETA, 1e-5, 0, None),
+    "layernorm_x": lambda lib: _layernorm(lib, x=X + 8),
+    "layernorm_y": lambda lib: _layernorm(lib, y=Y + 4),
+    "layernorm_xsum": lambda lib: _layernorm(lib, xsum=Z + 8, fvec=GAMMA + 0x200000),
+    "layernorm_y_narrow": lambda lib: _layernorm(lib, y=Y + 8, c=64),
+    "copy2d_src": lambda lib: lib.b200svd_copy2d(X + 8, 320, Y, 320, 4, 320, None),
+    "copy2d_dst": lambda lib: lib.b200svd_copy2d(X, 320, Y + 2, 320, 4, 320, None),
+    "add_rows_dst": lambda lib: lib.b200svd_add_rows(X + 8, 320, Y, 320, 4, 1, 320, None),
+    "add_rows_src": lambda lib: lib.b200svd_add_rows(X, 320, Y + 8, 320, 4, 4, 320, None),
+    "upsample2x_x": lambda lib: lib.b200svd_upsample2x(X + 8, Y, 1, 3, 5, 320, None),
+    "upsample2x_y": lambda lib: lib.b200svd_upsample2x(X, Y + 4, 1, 3, 5, 320, None),
+    "softmax_rows_in": lambda lib: lib.b200svd_softmax_rows(X + 8, 1000, Y, 1000, 3, 1000, None),
+    "softmax_rows_out": lambda lib: lib.b200svd_softmax_rows(X, 1000, Y + 4, 1000, 3, 1000, None),
+}
+
+
+@pytest.mark.parametrize("case", list(MISALIGNED))
+def test_norm_glue_reject_misaligned_bases(lib, case):
+    _assert_alignment_error(lib, MISALIGNED[case](lib))
+
+
+def _assert_error(lib, rc, *words):
+    msg = lib.b200svd_last_error().decode()
+    assert rc == 1, msg
+    for w in words:
+        assert w in msg, msg
+
+
+def test_layernorm_rejects_xsum_without_fvec(lib):
+    """xsum is bf16(x + fvec): without fvec the kernels would leave the caller's buffer unwritten."""
+    for c in (64, 320, 512):
+        _assert_error(lib, _layernorm(lib, xsum=Z, c=c), "xsum", "fvec")
+
+
+def test_layer_norm_wrapper_rejects_xsum_without_fvec(monkeypatch):
+    from streamingt2v_b200 import ops
+    monkeypatch.setattr(ops, "_call", lambda *a, **kw: pytest.fail("reached the library"))
+    x = torch.zeros(4, 64, dtype=torch.bfloat16)
+    with pytest.raises(AssertionError, match="fvec"):
+        ops.layer_norm(x, torch.ones(64), torch.zeros(64), xsum=torch.empty_like(x))
+
+
+def test_add_rows_rejects_empty_source(lib):
+    for src_rows in (0, -1):
+        _assert_error(lib, lib.b200svd_add_rows(X, 320, Y, 320, 4, src_rows, 320, None), "src_rows")
+
+
+GN_LIMITS = {
+    # p beyond the kernels' int row index, n beyond gridDim.y, c that cannot form 32 groups of whole vectors
+    "p_over_int_max": (1, 2 ** 31, 320, "p <="),
+    "n_over_65535": (65536, 16, 320, "n <= 65535"),
+    "negative_p": (1, -5, 320, "p <="),
+    "c_16": (1, 64, 16, "channel count"),
+    "c_8224": (1, 64, 8224, "channel count"),
+}
+
+
+@pytest.mark.parametrize("case", list(GN_LIMITS))
+def test_group_norm_rejects_shapes_it_cannot_index(lib, case):
+    n, p, c, word = GN_LIMITS[case]
+    assert lib.b200svd_gn_scratch_doubles(n, p, c) == -1
+    _assert_error(lib, lib.b200svd_gn_stats(X, c, n, p, c, Y, Z, Z + 0x100000, None), "gn_stats", word)
+    _assert_error(lib, lib.b200svd_gn_apply(X, c, Y, c, n, p, c, Z, GAMMA, BETA, 1e-5, 0, None), "gn_apply", word)
+
+
+def test_group_norm_partials_rejects_n_over_65535(lib):
+    _assert_error(lib, lib.b200svd_gn_stats_partials(X, Y, 64, 320, 320, 65536, Z, Z + 0x100000, Z + 0x200000, None),
+                  "gn_stats_partials", "n <= 65535")
+
+
+# zero elements: return 0 before any launch (the fake pointers are never touched)
+EMPTY = {
+    "layernorm_rows0": lambda lib: _layernorm(lib, rows=0),
+    "layernorm_rows0_narrow": lambda lib: _layernorm(lib, rows=0, c=64),
+    "layernorm_rows0_generic_fvec": lambda lib: _layernorm(lib, rows=0, c=512, xsum=Z, fvec=GAMMA + 0x200000),
+    "layernorm_c0": lambda lib: _layernorm(lib, c=0),
+    "softmax_rows": lambda lib: lib.b200svd_softmax_rows(X, 1000, Y, 1000, 0, 1000, None),
+    "softmax_cols": lambda lib: lib.b200svd_softmax_rows(X, 1000, Y, 1000, 3, 0, None),
+    "transpose_rows": lambda lib: lib.b200svd_transpose(X, 64, Y, 64, 0, 64, None),
+    "transpose_cols": lambda lib: lib.b200svd_transpose(X, 64, Y, 64, 64, 0, None),
+    "upsample2x": lambda lib: lib.b200svd_upsample2x(X, Y, 0, 3, 5, 320, None),
+    "upsample2x_h": lambda lib: lib.b200svd_upsample2x(X, Y, 2, 0, 5, 320, None),
+    "copy2d": lambda lib: lib.b200svd_copy2d(X, 320, Y, 320, 0, 320, None),
+    "add_rows": lambda lib: lib.b200svd_add_rows(X, 320, Y, 320, 0, 1, 320, None),
+    "add_silu": lambda lib: lib.b200svd_add_silu(X, Y, Z, 0, 1, None),
+    "nchw_to_nhwc": lambda lib: lib.b200svd_nchw_to_nhwc(X, 64, 0, 4, 64, Y, 8, 0, None),
+    "nchw_to_nhwc_hw": lambda lib: lib.b200svd_nchw_to_nhwc(X, 64, 3, 4, 0, Y, 8, 0, None),
+    "nhwc_to_nchw": lambda lib: lib.b200svd_nhwc_to_nchw(X, 0, 8, 0, 4, 64, Y, None),
+    "nhwc_to_nchw_c": lambda lib: lib.b200svd_nhwc_to_nchw(X, 1, 8, 3, 0, 64, Y, None),
+    "timestep_embed": lambda lib: lib.b200svd_timestep_embed(X, 0, 320, 10000.0, Y, 320, None),
+    "apm_mix": lambda lib: lib.b200svd_apm_mix(X, 0, 17, 1024, Y, Y, Y, Y, Y, Z, None),
+}
+
+
+@pytest.mark.parametrize("case", list(EMPTY))
+def test_empty_launch_returns_zero(lib, case):
+    rc = EMPTY[case](lib)
+    assert rc == 0, lib.b200svd_last_error().decode()
+
+
+_GN_EMPTY_SCRIPT = r"""
+import sys
+sys.path.insert(0, sys.argv[1])
+from streamingt2v_b200 import _lib
+lib = _lib.load()
+X, Y, Z = 0x7F0000000000, 0x7F0001000000, 0x7F0002000000
+for n, p in ((1, 0), (4, 0), (0, 100)):
+    assert lib.b200svd_gn_scratch_doubles(n, p, 320) == 0, (n, p)
+    assert lib.b200svd_gn_stats(X, 320, n, p, 320, Y, Z, Z + 4096, None) == 0, lib.b200svd_last_error()
+    assert lib.b200svd_gn_apply(X, 320, Y, 320, n, p, 320, Z, Y, Y, 1e-5, 1, None) == 0, lib.b200svd_last_error()
+for c in (0, -32):
+    assert lib.b200svd_gn_scratch_doubles(1, 64, c) == -1, c
+    assert lib.b200svd_gn_stats(X, 320, 1, 64, c, Y, Z, Z + 4096, None) == 1, c
+print("ok")
+"""
+
+
+def test_group_norm_empty_and_zero_width_in_subprocess(lib):
+    """p = 0 (or n = 0): nothing to normalise, return 0 without a launch.  c = 0: an error.  Both once reached an
+    integer division by zero in the host-side launch geometry, which kills the process; hence the subprocess."""
+    import os
+    import subprocess
+    import sys
+    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+    r = subprocess.run([sys.executable, "-c", _GN_EMPTY_SCRIPT, root], capture_output=True, text=True, timeout=300)
+    assert r.returncode == 0 and r.stdout.strip() == "ok", \
+        f"exit {r.returncode}\nstdout: {r.stdout[-2000:]}\nstderr: {r.stderr[-2000:]}"

@@ -27,53 +27,14 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from guard_bands import Guarded, _check_bound
+
 pytestmark = pytest.mark.gpu
 
-NAN = float("nan")
-
 
 # ---------------------------------------------------------------------------------------------------------------------
-# guard bands
+# guard bands (tests/guard_bands.py)
 # ---------------------------------------------------------------------------------------------------------------------
-class Guarded:
-    """`view` ([rows, cols]) sits at row `pre` of a NaN-filled [pre + rows + post, ld] buffer, ld = cols rounded up
-    to 8 plus `pad` columns.  `flat=True`: a contiguous tensor of any shape inside a flat NaN buffer instead."""
-
-    def __init__(self, shape, dtype, dev, *, pre=3, post=5, pad=8, flat=False):
-        assert pad % 8 == 0
-        self.dtype = dtype
-        if flat:
-            n = math.prod(shape)
-            self.buf = torch.full((8 * pre + n + 8 * post,), NAN, dtype=dtype, device=dev)
-            self.view = self.buf[8 * pre:8 * pre + n].view(shape)
-        else:
-            rows, cols = shape
-            ld = -(-cols // 8) * 8 + pad
-            self.buf = torch.full((pre + rows + post, ld), NAN, dtype=dtype, device=dev)
-            self.view = self.buf[pre:pre + rows, :cols]
-        assert self.view.data_ptr() % 16 == 0
-
-    def fill(self, values):
-        self.view.copy_(values)
-        return self
-
-    def snapshot(self):
-        self._snap = self.buf.clone()
-        return self
-
-    def check(self, name):
-        """Inside the view: finite.  Outside: bitwise what it was at snapshot()."""
-        assert torch.isfinite(self.view.float()).all(), f"{name}: unwritten or non-finite output elements"
-        idx = torch.arange(self.buf.numel(), device=self.buf.device).view(self.buf.shape)
-        inside = idx.as_strided(self.view.shape, self.view.stride(), self.view.storage_offset() - self.buf.storage_offset())
-        outside = torch.ones(self.buf.numel(), dtype=torch.bool, device=self.buf.device)
-        outside[inside.reshape(-1)] = False
-        ity = torch.int16 if self.buf.element_size() == 2 else torch.int32
-        now, was = self.buf.view(ity).reshape(-1)[outside], self._snap.view(ity).reshape(-1)[outside]
-        n_bad = (now != was).sum().item()
-        assert n_bad == 0, f"{name}: {n_bad} elements outside the output view were written"
-
-
 def _out(shape, dtype, dev, **kw):
     return Guarded(shape, dtype, dev, **kw).snapshot()
 
@@ -95,19 +56,6 @@ def _small_ints(t):
 # ---------------------------------------------------------------------------------------------------------------------
 # bounds
 # ---------------------------------------------------------------------------------------------------------------------
-def _check_bound(out, ref, bound, name, family, l2=2 ** -8):
-    """Every element within `bound`, relative L2 within `l2`; prints the margin (run with -s to see it)."""
-    out = out.double()
-    err = (out - ref).abs()
-    ratio = (err / bound).max().item()
-    rel_l2 = (err.norm() / ref.norm().clamp_min(1e-300)).item()
-    print(f"[{family}] {name}: max err/bound {ratio:.3f}, rel L2 {rel_l2:.3e}")
-    assert torch.isfinite(out).all(), f"{name}: non-finite output"
-    n_bad = (err > bound).sum().item()
-    assert n_bad == 0, f"{name}: {n_bad}/{err.numel()} elements beyond the derived bound (worst ratio {ratio:.3f})"
-    assert rel_l2 <= l2, f"{name}: relative L2 error {rel_l2:.3e} > {l2:.3e}"
-
-
 def _gemm_bound(ref, fp32, act_term=None):
     rms = ref.pow(2).mean().sqrt()
     b = (2 ** -20 if fp32 else 2 ** -8) * ref.abs() + 2 ** -12 * rms

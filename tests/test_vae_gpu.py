@@ -56,8 +56,9 @@ def test_softmax_rows_and_transpose(cuda_dev):
     x = torch.randn(77, 200, device=cuda_dev).to(torch.bfloat16)
     xt = ops.transpose(x)
     torch.cuda.synchronize()
-    ref = F.softmax(s, dim=-1)
-    assert (p.float() - ref).abs().max().item() <= 2 ** -8 * ref.max().item() + 1e-6
+    ref = F.softmax(s.double(), dim=-1)
+    # per element: bf16 rounding (2^-8 p) plus __expf and the fp32 row sum (2^-16 p at this logit spread)
+    assert ((p.double() - ref).abs() <= (2 ** -8 + 2 ** -16) * ref).all()
     assert torch.equal(xt, x.t().contiguous())
 
 
