@@ -102,9 +102,10 @@ int b200svd_gemm_pair_mode(int mode);
  *   0  cooperative everywhere: both warpgroups work on the same 128 x bn tile, 64 rows each.
  *   1  alternating wherever it exists: each warpgroup computes whole 128 x bn tiles, the CTA's tiles in turn, so one
  *      warpgroup's epilogue runs under the other's MMAs.  bf16 outputs written by TMA stores without gn_part, N tile
- *      at most 160: a 256-wide tile runs as 128-wide tiles, except GEGLU, whose tile is fixed by its weights.
+ *      at most 128: a 256-wide tile runs as 128-wide tiles, except GEGLU, whose tile is fixed by its weights; the
+ *      160-wide tile stays cooperative.
  *   2  (default) alternating for launches of at least 2 tiles per SM whose tiles are short (taps x K blocks x 2 x bn
- *      below 20000 tensor-core clocks) and bn other than 160, cooperative otherwise.
+ *      below 20000 tensor-core clocks), cooperative otherwise.
  * Both schedules give bitwise the same output. */
 int b200svd_gemm_schedule(int mode);
 

@@ -166,7 +166,7 @@ struct TileCfg {
 };
 
 // Alternating schedule: a consumer warpgroup holds the whole 128 x BN accumulator (BN registers per thread, so
-// BN <= 160) and stages 128-row sub-tiles (8 KB, two buffers per warpgroup); no GroupNorm partials.
+// BN <= 128) and stages 128-row sub-tiles (8 KB, two buffers per warpgroup); no GroupNorm partials.
 constexpr int ALT_STG_SLOT_BYTES = BM * SUB_W * 2;
 constexpr int ALT_STG_BYTES = 2 * STG_SLOTS * ALT_STG_SLOT_BYTES;
 template <int BN>
@@ -181,7 +181,7 @@ struct AltCfg {
   static constexpr int PRODUCER_REGS = 40;
   static constexpr int RES_SLOTS_AT_MIN = (SMEM_LIMIT - FIXED - MIN_STAGES * STAGE_BYTES) / RES_SLOT_BYTES;
   static int res_slots_fit(int stages) { return (SMEM_LIMIT - FIXED - stages * STAGE_BYTES) / RES_SLOT_BYTES; }
-  static_assert(BN <= 160, "128 x BN accumulator in one warpgroup's registers");
+  static_assert(BN <= 128, "128 x BN accumulator in one warpgroup's registers");
   static_assert(2 * 128 * CONSUMER_REGS + 128 * PRODUCER_REGS <= 65536, "register file");
   static_assert(STAGES >= 4, "pipeline depth without residuals");
   static_assert(RES_SLOTS_AT_MIN >= 2, "two residuals need two ring slots");
@@ -221,16 +221,17 @@ __device__ __forceinline__ void load_bf16_pair(const __nv_bfloat16* base, int64_
 
 // The epilogue arithmetic after bias and per-frame vector, shared by the fp32 and the bf16 output paths so that both
 // round the same fp32 value: activation (GEGLU: value * GELU(gate + gate bias), the gate bias already added), scale.
-// Multiplies and fused multiply-adds are written out so that the compiler cannot contract them differently.
-__device__ __forceinline__ float epi_act(const GemmDev& p, bool geglu, float v, float g) {
-  if (p.act == B200SVD_ACT_SILU) {
+// Multiplies and fused multiply-adds are written out so that the compiler cannot contract them differently.  An
+// activation known at compile time folds the tests away.
+__device__ __forceinline__ float epi_act(int act, float s_acc, float v, float g) {
+  if (act == B200SVD_ACT_SILU) {
     v = silu_fast(v);
-  } else if (p.act == B200SVD_ACT_GELU) {
+  } else if (act == B200SVD_ACT_GELU) {
     v = gelu_fast(v);
-  } else if (geglu) {
+  } else if (act == B200SVD_ACT_GEGLU) {
     v = __fmul_rn(v, gelu_fast(g));
   }
-  return __fmul_rn(v, p.s_acc);
+  return __fmul_rn(v, s_acc);
 }
 
 // byte offset of (row, 4-byte column pair `cp` of 16-byte chunk `ch`) in a 64-byte-row SWIZZLE_64B sub-tile buffer
@@ -238,16 +239,31 @@ __device__ __forceinline__ uint32_t sw64_off(uint32_t row, uint32_t ch, uint32_t
   return row * 64u + ((ch ^ ((row >> 1) & 3u)) << 4) + cp * 4u;
 }
 
-// ---- compile-time epilogue kinds of the staged bf16 output ----
-// The generic epilogue tests activation, bias, per-frame vector and residuals per element; those tests, and the global
-// loads sitting between them, are what a consumer warp spends its epilogue on.  The combinations the network launches
-// (b200svd_gemm_epilogue_kind) are compiled as branch-free bodies instead: one switch per tile picks the body.  Per
-// element the arithmetic is that of the generic body, operation for operation, so the output is bitwise the same.
+// ---- epilogue kinds of the staged bf16 output ----
+// Testing activation, bias, per-frame vector and residuals per element, and the global loads sitting between those
+// tests, is what a consumer warp would spend its epilogue on.  The combinations the network launches
+// (b200svd_gemm_epilogue_kind) are compiled as branch-free bodies instead, one switch per tile picking the body;
+// EpiGeneric reads the same flags from the launch parameters and keeps every other combination.  All of them run one
+// body (epi_stage_half), whose accessors are constants for a compiled kind, so per element the arithmetic is the same
+// operation for operation and the output is bitwise the same.
 template <int ACT_, bool BIAS_, bool FVEC_, int NRES_>
 struct Epi {
-  static constexpr int ACT = ACT_;
-  static constexpr bool BIAS = BIAS_, FVEC = FVEC_, GEGLU = ACT_ == B200SVD_ACT_GEGLU;
-  static constexpr int NRES = NRES_;
+  static constexpr bool GENERIC = false;
+  __device__ static int act(const GemmDev&) { return ACT_; }
+  __device__ static bool geglu(const GemmDev&) { return ACT_ == B200SVD_ACT_GEGLU; }
+  __device__ static bool bias(const GemmDev&) { return BIAS_; }
+  __device__ static bool fvec(const GemmDev&) { return FVEC_; }
+  __device__ static bool res1(const GemmDev&) { return NRES_ >= 1; }
+  __device__ static bool res2(const GemmDev&) { return NRES_ >= 2; }
+};
+struct EpiGeneric {
+  static constexpr bool GENERIC = true;
+  __device__ static int act(const GemmDev& p) { return p.act; }
+  __device__ static bool geglu(const GemmDev& p) { return p.act == B200SVD_ACT_GEGLU; }
+  __device__ static bool bias(const GemmDev& p) { return p.bias != nullptr; }
+  __device__ static bool fvec(const GemmDev& p) { return p.fvec != nullptr; }
+  __device__ static bool res1(const GemmDev& p) { return p.res1 != nullptr; }
+  __device__ static bool res2(const GemmDev& p) { return p.res2 != nullptr; }
 };
 // X(kind id, activation, bias, per-frame vector, residuals): what the two kernels instantiate
 #define MTGEMM_EPI_KINDS(X)                                    \
@@ -261,34 +277,45 @@ struct Epi {
   X(B200SVD_EPI_BIAS_SILU, B200SVD_ACT_SILU, true, false, 0)   \
   X(B200SVD_EPI_BIAS_GELU, B200SVD_ACT_GELU, true, false, 0)
 
-// epi_act with the activation known at compile time
-template <int ACT>
-__device__ __forceinline__ float epi_act_kind(float s_acc, float v, float g) {
-  if constexpr (ACT == B200SVD_ACT_SILU) v = silu_fast(v);
-  if constexpr (ACT == B200SVD_ACT_GELU) v = gelu_fast(v);
-  if constexpr (ACT == B200SVD_ACT_GEGLU) v = __fmul_rn(v, gelu_fast(g));
-  return __fmul_rn(v, s_acc);
-}
-
 // What a consumer thread knows about its tile
 struct EpiTile {
   uint32_t n0, otile0, n_out;  // first GEMM column, first output column, output width
   uint32_t mb1, mb2, mb3;      // row box origin
+  uint32_t mt;                 // M tile (the tile's GroupNorm partial-sum rows are 4 mt .. 4 mt + 3)
 };
+
+// Where row r (0-127) of the tile goes: whether it lies inside the output, its output row, and its per-frame vector
+// row (p.fvec itself for a row outside the output: any readable row will do, such a row is never stored).
+struct OutRow {
+  bool valid;
+  int64_t row;
+  const float* fv;
+};
+__device__ __forceinline__ OutRow out_row(const GemmDev& p, const EpiTile& t, uint32_t r) {
+  const uint32_t lb1 = p.m_lb[0], lb2 = p.m_lb[1];
+  const uint32_t m1 = t.mb1 + (r & ((1u << lb1) - 1));
+  const uint32_t m2 = t.mb2 + ((r >> lb1) & ((1u << lb2) - 1));
+  const uint32_t m3 = t.mb3 + (r >> (lb1 + lb2));
+  OutRow o;
+  o.valid = (m1 < p.m_ext[0]) && (m2 < p.m_ext[1]) && (m3 < p.m_ext[2]);
+  o.row = (int64_t)m1 * p.out_rs[0] + (int64_t)m2 * p.out_rs[1] + (int64_t)m3 * p.out_rs[2];
+  o.fv = p.fvec != nullptr && o.valid ? p.fvec + (int64_t)((uint32_t)o.row / p.rows_per_frame) * p.ldf : p.fvec;
+  return o;
+}
 
 // Bias and GEGLU gate bias of the thread's 8 columns of sub-tile c, loaded in one batch ahead of the residual waits
 // and the arithmetic.  Columns past the output width read nothing.
 template <int BN, class E>
 __device__ __forceinline__ void epi_load_bias(const GemmDev& p, const EpiTile& t, int c, uint32_t cq, float (&bv)[4][2],
                                               float (&gbv)[4][2]) {
-  if constexpr (E::BIAS) {
+  if (E::bias(p)) {
 #pragma unroll
     for (int jj = 0; jj < 4; ++jj) {
       const uint32_t tcol = (uint32_t)(8 * (4 * c + jj)) + 2 * cq;
 #pragma unroll
       for (int e = 0; e < 2; ++e) {
         bv[jj][e] = t.otile0 + tcol + e < t.n_out ? __ldg(p.bias + t.n0 + tcol + e) : 0.f;
-        if constexpr (E::GEGLU) gbv[jj][e] = __ldg(p.bias + t.n0 + BN / 2 + tcol + e);  // n is a multiple of BN
+        if (E::geglu(p)) gbv[jj][e] = __ldg(p.bias + t.n0 + BN / 2 + tcol + e);  // n is a multiple of BN
       }
     }
   }
@@ -296,24 +323,24 @@ __device__ __forceinline__ void epi_load_bias(const GemmDev& p, const EpiTile& t
 
 // One 64-row half of sub-tile c: the thread's rows rbase and rbase + 8 (of the 64), 8 columns each, from the m64nBN
 // accumulator fragment `acc` to the staging buffer `stg`; r1s / r2s are the residual sub-tiles of the same 64 rows.
-// fv[h] is the per-frame row of row h (any readable row if the row is outside the output: it is never stored); the
-// half's 16 per-frame values are loaded in one batch ahead of the arithmetic.
-// Order per element: bias, per-frame, gate bias, activation, s_acc, res1, res2, round.
+// rows[h] is where row h goes; the half's 16 per-frame values are loaded in one batch ahead of the arithmetic.
+// Order per element: bias, per-frame, gate bias, activation, s_acc, res1, res2, round.  An absent term is skipped,
+// not added as zero (-0 + 0 is +0).
 template <int BN, class E>
-__device__ __forceinline__ void epi_stage_half(const GemmDev& p, const EpiTile& t, const float (&acc)[BN / 2], int c,
+__device__ __forceinline__ void epi_stage_half(const GemmDev& p, const EpiTile& t, const float* acc, int c,
                                                uint32_t rbase, uint32_t cq, uint8_t* stg, const uint8_t* r1s,
                                                const uint8_t* r2s, const float (&bv)[4][2], const float (&gbv)[4][2],
-                                               const float* const (&fv)[2]) {
+                                               const OutRow (&rows)[2]) {
   constexpr int NJ = BN / 8;
   float fvv[2][4][2];
-  if constexpr (E::FVEC) {
+  if (E::fvec(p)) {
 #pragma unroll
     for (int h = 0; h < 2; ++h)
 #pragma unroll
       for (int jj = 0; jj < 4; ++jj) {
         const uint32_t ocol = t.otile0 + (uint32_t)(8 * (4 * c + jj)) + 2 * cq;
 #pragma unroll
-        for (int e = 0; e < 2; ++e) fvv[h][jj][e] = ocol + e < t.n_out ? __ldg(fv[h] + ocol + e) : 0.f;
+        for (int e = 0; e < 2; ++e) fvv[h][jj][e] = ocol + e < t.n_out ? __ldg(rows[h].fv + ocol + e) : 0.f;
       }
   }
 #pragma unroll
@@ -324,35 +351,106 @@ __device__ __forceinline__ void epi_stage_half(const GemmDev& p, const EpiTile& 
       const uint32_t off = sw64_off(rbase + 8u * h, (uint32_t)jj, cq);
       float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
       float g0 = 0.f, g1 = 0.f;
-      if constexpr (E::BIAS) {
+      if (E::bias(p)) {
         v0 += bv[jj][0];
         v1 += bv[jj][1];
       }
-      if constexpr (E::FVEC) {
+      if (E::fvec(p)) {
         v0 += fvv[h][jj][0];
         v1 += fvv[h][jj][1];
       }
-      if constexpr (E::GEGLU) {
-        g0 = acc[4 * (j + NJ / 2) + 2 * h];
-        g1 = acc[4 * (j + NJ / 2) + 2 * h + 1];
-        if constexpr (E::BIAS) {
-          g0 += gbv[jj][0];
-          g1 += gbv[jj][1];
+      // GEGLU launches only the 128- and 256-wide tiles, and only value columns (j < NJ / 2) reach here: the gate
+      // index stays inside the accumulator fragment at compile time.
+      if constexpr (BN == 128 || BN == 256) {
+        if (E::geglu(p) && j < NJ / 2) {
+          g0 = acc[4 * (j + NJ / 2) + 2 * h];
+          g1 = acc[4 * (j + NJ / 2) + 2 * h + 1];
+          if (E::bias(p)) {
+            g0 += gbv[jj][0];
+            g1 += gbv[jj][1];
+          }
         }
       }
-      v0 = epi_act_kind<E::ACT>(p.s_acc, v0, g0);
-      v1 = epi_act_kind<E::ACT>(p.s_acc, v1, g1);
-      if constexpr (E::NRES >= 1) {
+      v0 = epi_act(E::act(p), p.s_acc, v0, g0);
+      v1 = epi_act(E::act(p), p.s_acc, v1, g1);
+      if (E::res1(p)) {
         const uint32_t w = *reinterpret_cast<const uint32_t*>(r1s + off);
         v0 = __fmaf_rn(p.s1, bf16_lo(w), v0);
         v1 = __fmaf_rn(p.s1, bf16_hi(w), v1);
       }
-      if constexpr (E::NRES >= 2) {
+      if (E::res2(p)) {
         const uint32_t w = *reinterpret_cast<const uint32_t*>(r2s + off);
         v0 = __fmaf_rn(p.s2, bf16_lo(w), v0);
         v1 = __fmaf_rn(p.s2, bf16_hi(w), v1);
       }
       *reinterpret_cast<uint32_t*>(stg + off) = pack_bf16x2(v0, v1);
+    }
+  }
+}
+
+// GroupNorm partials of sub-tile c (cooperative generic launches with gn_part), summed from the bf16 words this
+// thread has just staged (the values the GroupNorm reads; the same thread wrote them, so no barrier is needed): column
+// sums over the warp's 16 rows (lanes of equal cq), then over the quadrant's two warps.  The odd warp of the quadrant
+// hands its sums to the even one through gxb; the even one parks its own in the accumulators of the sub-tile, which
+// are consumed, until gn_write_partials.
+template <int BN>
+__device__ __forceinline__ void gn_sum_partials(const EpiTile& t, float* acc, int c, uint32_t rbase, uint32_t cq,
+                                                const uint8_t* stg, const OutRow (&rows)[2], float* gxb, bool sender,
+                                                bool first_row) {
+  // every staged word is read back first, outside the tests, so that the reads overlap the shuffles
+  uint32_t sw[4][2];
+#pragma unroll
+  for (int jj = 0; jj < 4; ++jj)
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+      sw[jj][h] = *reinterpret_cast<const uint32_t*>(stg + sw64_off(rbase + 8u * h, (uint32_t)jj, cq));
+#pragma unroll
+  for (int jj = 0; jj < 4; ++jj) {
+    const int j = 4 * c + jj;
+    const uint32_t ocol = t.otile0 + (uint32_t)(8 * j) + 2 * cq;
+    const bool in0 = ocol < t.n_out, in1 = ocol + 1 < t.n_out;
+    float gs0 = 0.f, gs1 = 0.f, gq0 = 0.f, gq1 = 0.f;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      if (rows[h].valid && in0) {
+        const uint32_t w = sw[jj][h];
+        const float r0 = bf16_lo(w), r1 = in1 ? bf16_hi(w) : 0.f;
+        gs0 += r0;
+        gs1 += r1;
+        gq0 = __fmaf_rn(r0, r0, gq0);
+        gq1 = __fmaf_rn(r1, r1, gq1);
+      }
+    }
+#pragma unroll
+    for (int o = 4; o < 32; o <<= 1) {
+      gs0 += __shfl_xor_sync(0xffffffffu, gs0, o);
+      gs1 += __shfl_xor_sync(0xffffffffu, gs1, o);
+      gq0 += __shfl_xor_sync(0xffffffffu, gq0, o);
+      gq1 += __shfl_xor_sync(0xffffffffu, gq1, o);
+    }
+    if (sender && first_row) *reinterpret_cast<float4*>(gxb + 2 * (8 * jj + 2 * cq)) = make_float4(gs0, gq0, gs1, gq1);
+    if (!sender) {
+      acc[4 * j] = gs0;
+      acc[4 * j + 1] = gq0;
+      acc[4 * j + 2] = gs1;
+      acc[4 * j + 3] = gq1;
+    }
+  }
+}
+
+// After the named barrier: the even warp of the quadrant adds the partner's sums from gxb to its own and writes the
+// quadrant's partials of sub-tile c to partial-sum row `slot`.
+__device__ __forceinline__ void gn_write_partials(const GemmDev& p, const EpiTile& t, const float* acc, int c,
+                                                  uint32_t cq, const float* gxb, uint32_t slot) {
+  float2* dst = reinterpret_cast<float2*>(p.gn_part) + (int64_t)slot * p.gn_ld;
+#pragma unroll
+  for (int jj = 0; jj < 4; ++jj) {
+    const int j = 4 * c + jj;
+    const uint32_t ocol = t.otile0 + (uint32_t)(8 * j) + 2 * cq;
+    if (ocol < t.n_out) {
+      const float4 o = *reinterpret_cast<const float4*>(gxb + 2 * (8 * jj + 2 * cq));
+      dst[ocol] = make_float2(acc[4 * j] + o.x, acc[4 * j + 1] + o.y);
+      if (ocol + 1 < t.n_out) dst[ocol + 1] = make_float2(acc[4 * j + 2] + o.z, acc[4 * j + 3] + o.w);
     }
   }
 }
@@ -427,98 +525,54 @@ __device__ __forceinline__ void produce_residuals(const GemmDev& p, const CUtens
   }
 }
 
-// The staged bf16 epilogue of one tile on the cooperative schedule for epilogue kind E: the sub-tile loop of
-// mtgemm_kernel with the same waits, barrier and store order, the element loop replaced by epi_stage_half.
-template <int BN, class E>
-__device__ __forceinline__ void coop_epilogue_kind(const GemmDev& p, const CUtensorMap* tmO, const EpiTile& t,
-                                                   const float (&acc)[BN / 2], uint8_t* stg_smem,
-                                                   const uint8_t* res_smem, uint64_t* res_full, uint64_t* res_empty,
-                                                   uint32_t rslots, uint32_t& rslot, uint32_t& rph, uint32_t& stg_it,
-                                                   int cw, uint32_t rbase, uint32_t cq, bool leader,
-                                                   const float* const (&fv)[2], PhaseClock& pc) {
-  constexpr int NSUB = (E::GEGLU ? BN / 2 : BN) / SUB_W;  // gate columns are consumed with their value columns
+// The staged bf16 epilogue of one tile for epilogue kind E on either schedule.  A consumer warpgroup holds HALVES
+// 64-row halves of the tile: 1 on the cooperative schedule (its own 64 rows, 4 KB staging slots, its rows of each
+// residual slot at cw * STG_SLOT_BYTES, stores at the box origin moved by wg_off), 2 on the alternating one (the whole
+// tile, 8 KB slots, stores at the tile's box).  Sub-tile by sub-tile: bias loads, the residual waits in the order the
+// residual producer loads them, the arithmetic into one of the warpgroup's two staging slots, and one TMA store once
+// the store issued a sub-tile ago has read the other slot.  gn_x is the GroupNorm exchange area (cooperative only).
+template <int BN, class E, int HALVES>
+__device__ __forceinline__ void epilogue_staged(const GemmDev& p, const CUtensorMap* tmO, const EpiTile& t,
+                                                float* const (&acc)[HALVES], const OutRow (&rows)[HALVES][2],
+                                                uint8_t* stg_smem, const uint8_t* res_smem, uint64_t* res_full,
+                                                uint64_t* res_empty, RingPos& rr, uint32_t& stg_it, uint32_t cw,
+                                                uint32_t rbase, uint32_t cq, bool leader, float* gn_x, PhaseClock& pc) {
+  constexpr uint32_t SLOT_BYTES = HALVES * STG_SLOT_BYTES;
+  const uint8_t* res_rows = res_smem + (HALVES == 1 ? cw * STG_SLOT_BYTES : 0u);
+  const uint32_t wl = rbase >> 4, rq = rbase & 7u;  // warp of the warpgroup, row of the lane in its 8-row group
 #pragma unroll
-  for (int c = 0; c < NSUB; ++c) {
+  for (int c = 0; c < BN / SUB_W; ++c) {
+    if (E::geglu(p) && c >= BN / SUB_W / 2) break;  // gate columns are consumed with their value columns
     if (t.otile0 + (uint32_t)(c * SUB_W) >= t.n_out) break;
-    uint8_t* stg = stg_smem + (cw * STG_SLOTS + (stg_it & 1)) * STG_SLOT_BYTES;
+    uint8_t* stg = stg_smem + (cw * STG_SLOTS + (stg_it & 1)) * SLOT_BYTES;
     float bv[4][2], gbv[4][2];
     epi_load_bias<BN, E>(p, t, c, cq, bv, gbv);
-    const uint8_t* r1s = res_smem;
-    const uint8_t* r2s = res_smem;
+    const uint8_t* r1s = res_rows;
+    const uint8_t* r2s = res_rows;
     uint32_t r1slot = 0, r2slot = 0;
     pc.mark(PC_EPI);
-    if constexpr (E::NRES >= 1) {
-      r1slot = rslot;
-      mbar_wait(&res_full[rslot], rph);
-      r1s = res_smem + rslot * RES_SLOT_BYTES + cw * STG_SLOT_BYTES;
-      if (++rslot == rslots) {
-        rslot = 0;
-        rph ^= 1;
-      }
-    }
-    if constexpr (E::NRES >= 2) {
-      r2slot = rslot;
-      mbar_wait(&res_full[rslot], rph);
-      r2s = res_smem + rslot * RES_SLOT_BYTES + cw * STG_SLOT_BYTES;
-      if (++rslot == rslots) {
-        rslot = 0;
-        rph ^= 1;
-      }
-    }
-    pc.mark(PC_RES_WAIT);
-    epi_stage_half<BN, E>(p, t, acc, c, rbase, cq, stg, r1s, r2s, bv, gbv, fv);
-    fence_proxy_async_smem();  // the staged values are read by the TMA store (async proxy)
-    // the store issued one sub-tile ago has read the other staging buffer: it may be refilled next sub-tile
-    pc.mark(PC_EPI);
-    if (leader) tma_store_wait_read0();
-    named_bar_sync(5 + cw, 128);
-    pc.mark(PC_STORE_WAIT);
-    if (leader) {
-      if constexpr (E::NRES >= 1) mbar_arrive(&res_empty[r1slot]);
-      if constexpr (E::NRES >= 2) mbar_arrive(&res_empty[r2slot]);
-      tma_store_4d(tmO, stg, (int)(t.otile0 + c * SUB_W), (int)(t.mb1 + (cw ? p.wg_off[0] : 0u)),
-                   (int)(t.mb2 + (cw ? p.wg_off[1] : 0u)), (int)(t.mb3 + (cw ? p.wg_off[2] : 0u)));
-      tma_store_commit();
-    }
-    ++stg_it;
-  }
-}
-
-// The same for the alternating schedule: the warpgroup holds both 64-row halves of the tile.
-template <int BN, class E>
-__device__ __forceinline__ void alt_epilogue_kind(const GemmDev& p, const CUtensorMap* tmO, const EpiTile& t,
-                                                  const float (&acc0)[BN / 2], const float (&acc1)[BN / 2],
-                                                  uint8_t* stg_smem, const uint8_t* res_smem, uint64_t* res_full,
-                                                  uint64_t* res_empty, uint32_t rslots, RingPos& rr, uint32_t& stg_it,
-                                                  uint32_t cw, uint32_t rbase, uint32_t cq, bool leader,
-                                                  const float* const (&fv)[2][2], PhaseClock& pc) {
-  constexpr int NSUB = (E::GEGLU ? BN / 2 : BN) / SUB_W;
-  constexpr uint32_t HALF = 64 * SUB_W * 2;  // bytes of a 64-row half of a sub-tile; the swizzle repeats every 8 rows
-#pragma unroll
-  for (int c = 0; c < NSUB; ++c) {
-    if (t.otile0 + (uint32_t)(c * SUB_W) >= t.n_out) break;
-    uint8_t* stg = stg_smem + (cw * STG_SLOTS + (stg_it & 1)) * ALT_STG_SLOT_BYTES;
-    float bv[4][2], gbv[4][2];
-    epi_load_bias<BN, E>(p, t, c, cq, bv, gbv);
-    const uint8_t* r1s = res_smem;
-    const uint8_t* r2s = res_smem;
-    uint32_t r1slot = 0, r2slot = 0;
-    pc.mark(PC_EPI);
-    if constexpr (E::NRES >= 1) {
+    if (E::res1(p)) {
       r1slot = rr.idx;
       mbar_wait(&res_full[rr.idx], rr.phase);
-      r1s = res_smem + rr.idx * RES_SLOT_BYTES;
-      ring_step(rr, rslots);
+      r1s = res_rows + rr.idx * RES_SLOT_BYTES;
+      ring_step(rr, p.res_slots);
     }
-    if constexpr (E::NRES >= 2) {
+    if (E::res2(p)) {
       r2slot = rr.idx;
       mbar_wait(&res_full[rr.idx], rr.phase);
-      r2s = res_smem + rr.idx * RES_SLOT_BYTES;
-      ring_step(rr, rslots);
+      r2s = res_rows + rr.idx * RES_SLOT_BYTES;
+      ring_step(rr, p.res_slots);
     }
     pc.mark(PC_RES_WAIT);
-    epi_stage_half<BN, E>(p, t, acc0, c, rbase, cq, stg, r1s, r2s, bv, gbv, fv[0]);
-    epi_stage_half<BN, E>(p, t, acc1, c, rbase, cq, stg + HALF, r1s + HALF, r2s + HALF, bv, gbv, fv[1]);
+#pragma unroll
+    for (int hh = 0; hh < HALVES; ++hh)
+      epi_stage_half<BN, E>(p, t, acc[hh], c, rbase, cq, stg + hh * STG_SLOT_BYTES, r1s + hh * STG_SLOT_BYTES,
+                            r2s + hh * STG_SLOT_BYTES, bv, gbv, rows[hh]);
+    float* gxb = nullptr;
+    if constexpr (HALVES == 1 && E::GENERIC) {
+      gxb = gn_x + ((cw * 2 + (stg_it & 1)) * 2 + (wl >> 1)) * (SUB_W * 2);
+      if (p.gn_part != nullptr) gn_sum_partials<BN>(t, acc[0], c, rbase, cq, stg, rows[0], gxb, wl & 1, rq == 0);
+    }
     fence_proxy_async_smem();  // the staged values are read by the TMA store (async proxy)
     pc.mark(PC_EPI);
     // the store issued one sub-tile ago has read the other staging buffer: it may be refilled next sub-tile
@@ -526,10 +580,17 @@ __device__ __forceinline__ void alt_epilogue_kind(const GemmDev& p, const CUtens
     named_bar_sync(5 + (int)cw, 128);
     pc.mark(PC_STORE_WAIT);
     if (leader) {
-      if constexpr (E::NRES >= 1) mbar_arrive(&res_empty[r1slot]);
-      if constexpr (E::NRES >= 2) mbar_arrive(&res_empty[r2slot]);
-      tma_store_4d(tmO, stg, (int)(t.otile0 + c * SUB_W), (int)t.mb1, (int)t.mb2, (int)t.mb3);  // the tile's row box
+      if (E::res1(p)) mbar_arrive(&res_empty[r1slot]);
+      if (E::res2(p)) mbar_arrive(&res_empty[r2slot]);
+      // cooperative: the warpgroup's 64 rows, the tile's row box halved in its outermost non-unit dimension
+      const bool second = HALVES == 1 && cw != 0;
+      tma_store_4d(tmO, stg, (int)(t.otile0 + c * SUB_W), (int)(t.mb1 + (second ? p.wg_off[0] : 0u)),
+                   (int)(t.mb2 + (second ? p.wg_off[1] : 0u)), (int)(t.mb3 + (second ? p.wg_off[2] : 0u)));
       tma_store_commit();
+    }
+    if constexpr (HALVES == 1 && E::GENERIC) {
+      if (p.gn_part != nullptr && (wl & 1) == 0 && rq == 0)
+        gn_write_partials(p, t, acc[0], c, cq, gxb, t.mt * 4u + 2 * cw + (wl >> 1));
     }
     ++stg_it;
   }
@@ -593,13 +654,10 @@ mtgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
   const int wl = warp & 3;  // warp of the warpgroup: rows 16 wl .. 16 wl + 15 of those 64
   const int rq = lane >> 2, cq = lane & 3;
   const bool leader = (threadIdx.x & 127) == 0;
-  const uint32_t lb1 = p.m_lb[0], lb2 = p.m_lb[1];
-  const int quad = 2 * cw + (wl >> 1);  // 32-row quadrant of the tile
-  const bool gn = p.gn_part != nullptr;
-  const bool gn_sender = (wl & 1) != 0;
-  uint32_t st = 0, sph = 0;         // A/B ring position
-  uint32_t rslot = 0, rph = 0;      // residual ring position
-  uint32_t stg_it = 0;              // sub-tiles staged by this warpgroup so far
+  const uint32_t rbase = (uint32_t)(16 * wl + rq);
+  RingPos ab = {0, 0};   // A/B ring position
+  RingPos rr = {0, 0};   // residual ring position
+  uint32_t stg_it = 0;   // sub-tiles staged by this warpgroup so far
   float acc[R];
   PhaseClock pc;
 
@@ -609,9 +667,9 @@ mtgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
     for (int i = 0; i < R; ++i) acc[i] = 0.f;
     uint32_t prev = 0;
     for (uint32_t i = 0; i < iters_per_tile; ++i) {
-      mbar_wait(&full_bar[st], sph);
+      mbar_wait(&full_bar[ab.idx], ab.phase);
       pc.mark(PC_RING_WAIT);
-      const uint32_t sa = smem_u32(smem + st * Cfg::STAGE_BYTES);
+      const uint32_t sa = smem_u32(smem + ab.idx * Cfg::STAGE_BYTES);
       const uint64_t adesc = smem_desc_k_sw128(sa + cw * (A_STAGE_BYTES / 2));
       const uint64_t bdesc = smem_desc_k_sw128(sa + A_STAGE_BYTES);
       wgmma_fence_regs(acc);
@@ -625,11 +683,8 @@ mtgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
       wgmma_wait<1>();
       pc.mark(PC_MMA);
       if (i > 0 && leader) mbar_arrive(&empty_bar[prev]);
-      prev = st;
-      if (++st == stages) {
-        st = 0;
-        sph ^= 1;
-      }
+      prev = ab.idx;
+      ring_step(ab, stages);
     }
     wgmma_wait<0>();
     pc.mark(PC_MMA);
@@ -639,244 +694,89 @@ mtgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
     // ----- epilogue: thread holds rows r0 and r0 + 8, columns 8 j + 2 cq + {0, 1} (acc[4 j + 2 h + e]) -----
     uint32_t n_tile, mb1, mb2, mb3;
     decode_tile(p, tile, n_tile, mb1, mb2, mb3);
-    const uint32_t n0 = n_tile * BN;
-    const uint32_t otile0 = n_tile * tile_out_w;
-    bool valid[2];
-    int64_t row[2];
-    const float* fv[2];
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const uint32_t r = (uint32_t)(64 * cw + 16 * wl + rq + 8 * h);
-      const uint32_t m1 = mb1 + (r & ((1u << lb1) - 1));
-      const uint32_t m2 = mb2 + ((r >> lb1) & ((1u << lb2) - 1));
-      const uint32_t m3 = mb3 + (r >> (lb1 + lb2));
-      valid[h] = (m1 < p.m_ext[0]) && (m2 < p.m_ext[1]) && (m3 < p.m_ext[2]);
-      row[h] = (int64_t)m1 * p.out_rs[0] + (int64_t)m2 * p.out_rs[1] + (int64_t)m3 * p.out_rs[2];
-      fv[h] = (p.fvec != nullptr && valid[h]) ? p.fvec + (int64_t)((uint32_t)row[h] / p.rows_per_frame) * p.ldf
-                                              : nullptr;
-    }
-    constexpr int NJ = BN / 8;
-    if (p.epi_kind != B200SVD_EPI_GENERIC) {
-      // ----- staged bf16 output, epilogue kind known at compile time (launch-uniform: one switch per tile) -----
-      const EpiTile et = {n0, otile0, n_out, mb1, mb2, mb3};
-      const float* const fvk[2] = {fv[0] != nullptr ? fv[0] : p.fvec, fv[1] != nullptr ? fv[1] : p.fvec};
-      const uint32_t rbase = (uint32_t)(16 * wl + rq);
+    const EpiTile et = {n_tile * BN, n_tile * tile_out_w, n_out, mb1, mb2, mb3, tile / p.n_tiles};
+    const OutRow rows[1][2] = {{out_row(p, et, 64 * cw + rbase), out_row(p, et, 64 * cw + rbase + 8)}};
+    if (p.staged) {
+      // ----- bf16 output: 32-column sub-tiles staged in shared memory (SWIZZLE_64B, conflict-free fragment
+      // writes), written by one TMA store per warpgroup and sub-tile; residuals come from the TMA-fed ring.  The
+      // epilogue kind is launch-uniform: one switch per tile -----
+      float* const accs[1] = {acc};
       switch (p.epi_kind) {
+        case B200SVD_EPI_GENERIC:
+          epilogue_staged<BN, EpiGeneric, 1>(p, &tmO, et, accs, rows, stg_smem, res_smem, res_full, res_empty, rr,
+                                             stg_it, cw, rbase, cq, leader, gn_x, pc);
+          break;
 #define MTGEMM_CASE(ID, ACT, BIAS, FVEC, NRES)                                                                    \
   case ID:                                                                                                        \
     if constexpr (ACT != B200SVD_ACT_GEGLU || BN == 128 || BN == 256)                                             \
-      coop_epilogue_kind<BN, Epi<ACT, BIAS, FVEC, NRES>>(p, &tmO, et, acc, stg_smem, res_smem, res_full,          \
-                                                         res_empty, rslots, rslot, rph, stg_it, cw, rbase,        \
-                                                         (uint32_t)cq, leader, fvk, pc);                          \
+      epilogue_staged<BN, Epi<ACT, BIAS, FVEC, NRES>, 1>(p, &tmO, et, accs, rows, stg_smem, res_smem, res_full,   \
+                                                         res_empty, rr, stg_it, cw, rbase, cq, leader, gn_x, pc); \
     break;
         MTGEMM_EPI_KINDS(MTGEMM_CASE)
 #undef MTGEMM_CASE
       }
-      continue;
-    }
-    if (p.staged) {
-      // ----- bf16 output: 32-column sub-tiles staged in shared memory (SWIZZLE_64B, conflict-free fragment
-      // writes), written by one TMA store per warpgroup and sub-tile; residuals come from the TMA-fed ring -----
-#pragma unroll
-      for (int c = 0; c < Cfg::SUBTILES; ++c) {
-        if (geglu && c >= Cfg::SUBTILES / 2) break;  // gate columns are consumed with their value columns
-        if (otile0 + (uint32_t)(c * SUB_W) >= n_out) break;
-        uint8_t* stg = stg_smem + (cw * STG_SLOTS + (stg_it & 1)) * STG_SLOT_BYTES;
-        float* gxb = gn_x + ((cw * 2 + (stg_it & 1)) * 2 + (wl >> 1)) * (SUB_W * 2);
-        // residual sub-tiles of this warpgroup's 64 rows, in the order the residual producer loads them
-        const uint8_t* r1s = nullptr;
-        const uint8_t* r2s = nullptr;
-        uint32_t r1slot = 0, r2slot = 0;
-        pc.mark(PC_EPI);
-        if (p.res1 != nullptr) {
-          r1slot = rslot;
-          mbar_wait(&res_full[rslot], rph);
-          r1s = res_smem + rslot * RES_SLOT_BYTES + cw * STG_SLOT_BYTES;
-          if (++rslot == rslots) {
-            rslot = 0;
-            rph ^= 1;
-          }
-        }
-        if (p.res2 != nullptr) {
-          r2slot = rslot;
-          mbar_wait(&res_full[rslot], rph);
-          r2s = res_smem + rslot * RES_SLOT_BYTES + cw * STG_SLOT_BYTES;
-          if (++rslot == rslots) {
-            rslot = 0;
-            rph ^= 1;
-          }
-        }
-        pc.mark(PC_RES_WAIT);
-#pragma unroll
-        for (int jj = 0; jj < 4; ++jj) {
-          const int j = 4 * c + jj;
-          const uint32_t tcol = (uint32_t)(8 * j + 2 * cq);
-          const uint32_t ocol = otile0 + tcol;
-          const bool in0 = ocol < n_out, in1 = ocol + 1 < n_out;
-          float gs0 = 0.f, gs1 = 0.f, gq0 = 0.f, gq1 = 0.f;  // GroupNorm partials of the two columns
-          // bias, gate bias and per-frame values of the column pair, loaded together ahead of the arithmetic
-          float bv[2], gbv[2], fvv[2][2];
-#pragma unroll
-          for (int e = 0; e < 2; ++e) {
-            const bool in = e == 0 ? in0 : in1;
-            bv[e] = (p.bias != nullptr && in) ? __ldg(p.bias + n0 + tcol + e) : 0.f;
-            gbv[e] = (geglu && p.bias != nullptr) ? __ldg(p.bias + n0 + BN / 2 + tcol + e) : 0.f;
-#pragma unroll
-            for (int h = 0; h < 2; ++h) fvv[h][e] = (fv[h] != nullptr && in) ? __ldg(fv[h] + ocol + e) : 0.f;
-          }
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            const uint32_t off = sw64_off((uint32_t)(16 * wl + rq + 8 * h), (uint32_t)jj, (uint32_t)cq);
-            float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
-            float g0 = 0.f, g1 = 0.f;
-            if (p.bias != nullptr) {
-              v0 += bv[0];
-              v1 += bv[1];
-            }
-            if (fv[h] != nullptr) {
-              v0 += fvv[h][0];
-              v1 += fvv[h][1];
-            }
-            if (geglu) {
-              g0 = acc[4 * (j + NJ / 2) + 2 * h];
-              g1 = acc[4 * (j + NJ / 2) + 2 * h + 1];
-              if (p.bias != nullptr) {
-                g0 += gbv[0];
-                g1 += gbv[1];
-              }
-            }
-            v0 = epi_act(p, geglu, v0, g0);
-            v1 = epi_act(p, geglu, v1, g1);
-            if (r1s != nullptr) {
-              const uint32_t w = *reinterpret_cast<const uint32_t*>(r1s + off);
-              v0 = __fmaf_rn(p.s1, bf16_lo(w), v0);
-              v1 = __fmaf_rn(p.s1, bf16_hi(w), v1);
-            }
-            if (r2s != nullptr) {
-              const uint32_t w = *reinterpret_cast<const uint32_t*>(r2s + off);
-              v0 = __fmaf_rn(p.s2, bf16_lo(w), v0);
-              v1 = __fmaf_rn(p.s2, bf16_hi(w), v1);
-            }
-            const uint32_t w = pack_bf16x2(v0, v1);
-            *reinterpret_cast<uint32_t*>(stg + off) = w;
-            if (gn && valid[h] && in0) {
-              // statistics of the bf16-ROUNDED values, the ones the consumer reads
-              const float r0 = bf16_lo(w), r1 = in1 ? bf16_hi(w) : 0.f;
-              gs0 += r0;
-              gs1 += r1;
-              gq0 = __fmaf_rn(r0, r0, gq0);
-              gq1 = __fmaf_rn(r1, r1, gq1);
-            }
-          }
-          if (gn) {
-            // column sums over the warp's 16 rows (lanes of equal cq), then over the quadrant's two warps via smem
-#pragma unroll
-            for (int o = 4; o < 32; o <<= 1) {
-              gs0 += __shfl_xor_sync(0xffffffffu, gs0, o);
-              gs1 += __shfl_xor_sync(0xffffffffu, gs1, o);
-              gq0 += __shfl_xor_sync(0xffffffffu, gq0, o);
-              gq1 += __shfl_xor_sync(0xffffffffu, gq1, o);
-            }
-            if (gn_sender && rq == 0)
-              *reinterpret_cast<float4*>(gxb + 2 * (8 * jj + 2 * cq)) = make_float4(gs0, gq0, gs1, gq1);
-            if (!gn_sender) {
-              acc[4 * j] = gs0;  // the accumulators of this column block are consumed: park the partials there
-              acc[4 * j + 1] = gq0;
-              acc[4 * j + 2] = gs1;
-              acc[4 * j + 3] = gq1;
-            }
-          }
-        }
-        fence_proxy_async_smem();  // the staged values are read by the TMA store (async proxy)
-        // the store issued one sub-tile ago has read the other staging buffer: it may be refilled next sub-tile
-        pc.mark(PC_EPI);
-        if (leader) tma_store_wait_read0();
-        named_bar_sync(5 + cw, 128);
-        pc.mark(PC_STORE_WAIT);
-        if (leader) {
-          if (r1s != nullptr) mbar_arrive(&res_empty[r1slot]);
-          if (r2s != nullptr) mbar_arrive(&res_empty[r2slot]);
-          // the warpgroup's 64 rows: the tile's row box halved in its outermost non-unit dimension
-          tma_store_4d(&tmO, stg, (int)(otile0 + c * SUB_W), (int)(mb1 + (cw ? p.wg_off[0] : 0u)),
-                       (int)(mb2 + (cw ? p.wg_off[1] : 0u)), (int)(mb3 + (cw ? p.wg_off[2] : 0u)));
-          tma_store_commit();
-        }
-        if (gn && !gn_sender && rq == 0) {
-          const uint32_t slot = (tile / p.n_tiles) * 4u + (uint32_t)quad;
-          float2* dst = reinterpret_cast<float2*>(p.gn_part) + (int64_t)slot * p.gn_ld;
-#pragma unroll
-          for (int jj = 0; jj < 4; ++jj) {
-            const int j = 4 * c + jj;
-            const uint32_t ocol = otile0 + (uint32_t)(8 * j + 2 * cq);
-            if (ocol < n_out) {
-              const float4 o = *reinterpret_cast<const float4*>(gxb + 2 * (8 * jj + 2 * cq));
-              dst[ocol] = make_float2(acc[4 * j] + o.x, acc[4 * j + 1] + o.y);
-              if (ocol + 1 < n_out) dst[ocol + 1] = make_float2(acc[4 * j + 2] + o.z, acc[4 * j + 3] + o.w);
-            }
-          }
-        }
-        ++stg_it;
-      }
-      if (gn && !gn_sender && lane == 0 && n_tile == 0) {
+      if (p.gn_part != nullptr && (wl & 1) == 0 && lane == 0 && n_tile == 0) {
         // lane 0 holds the first row of the quadrant: if it is out of range, so is every row of the quadrant
-        const uint32_t slot = (tile / p.n_tiles) * 4u + (uint32_t)quad;
-        p.gn_slot_sample[slot] = valid[0] ? (int32_t)((uint32_t)row[0] / p.gn_rows) : -1;
+        const uint32_t slot = et.mt * 4u + (uint32_t)(2 * cw + (wl >> 1));
+        p.gn_slot_sample[slot] = rows[0][0].valid ? (int32_t)((uint32_t)rows[0][0].row / p.gn_rows) : -1;
       }
       continue;
     }
     // ----- fp32 output (pitches a tensor map cannot describe), or a bf16 output whose width is not a whole number
     // of 16-byte chunks (a TMA store writes whole chunks): straight from the accumulator registers -----
+    constexpr int NJ = BN / 8;
 #pragma unroll
     for (int j = 0; j < NJ; ++j) {
       if (geglu && j >= NJ / 2) break;  // gate columns are consumed with their value columns
       const uint32_t tcol = 8 * j + 2 * cq;  // column in the tile (value column for GEGLU)
-      const uint32_t ocol = otile0 + tcol;
+      const uint32_t ocol = et.otile0 + tcol;
       const bool in0 = ocol < n_out, in1 = ocol + 1 < n_out;
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
-        if (!valid[h] || !in0) continue;
+        if (!rows[0][h].valid || !in0) continue;
+        const int64_t row = rows[0][h].row;
         if (p.bias != nullptr) {
-          v0 += __ldg(p.bias + n0 + tcol);
-          if (in1) v1 += __ldg(p.bias + n0 + tcol + 1);
+          v0 += __ldg(p.bias + et.n0 + tcol);
+          if (in1) v1 += __ldg(p.bias + et.n0 + tcol + 1);
         }
-        if (fv[h] != nullptr) {
-          v0 += __ldg(fv[h] + ocol);
-          if (in1) v1 += __ldg(fv[h] + ocol + 1);
+        if (p.fvec != nullptr) {
+          v0 += __ldg(rows[0][h].fv + ocol);
+          if (in1) v1 += __ldg(rows[0][h].fv + ocol + 1);
         }
         float g0 = 0.f, g1 = 0.f;
         if (geglu) {
           g0 = acc[4 * (j + NJ / 2) + 2 * h];
           g1 = acc[4 * (j + NJ / 2) + 2 * h + 1];
           if (p.bias != nullptr) {
-            g0 += __ldg(p.bias + n0 + BN / 2 + tcol);
-            if (in1) g1 += __ldg(p.bias + n0 + BN / 2 + tcol + 1);
+            g0 += __ldg(p.bias + et.n0 + BN / 2 + tcol);
+            if (in1) g1 += __ldg(p.bias + et.n0 + BN / 2 + tcol + 1);
           }
         }
-        v0 = epi_act(p, geglu, v0, g0);
-        v1 = epi_act(p, geglu, v1, g1);
+        v0 = epi_act(p.act, p.s_acc, v0, g0);
+        v1 = epi_act(p.act, p.s_acc, v1, g1);
         if (p.res1 != nullptr) {
           float a, b;
-          load_bf16_pair(p.res1, row[h] * p.ld1 + ocol, in1, a, b);
+          load_bf16_pair(p.res1, row * p.ld1 + ocol, in1, a, b);
           v0 = __fmaf_rn(p.s1, a, v0);
           v1 = __fmaf_rn(p.s1, b, v1);
         }
         if (p.res2 != nullptr) {
           float a, b;
-          load_bf16_pair(p.res2, row[h] * p.ld2 + ocol, in1, a, b);
+          load_bf16_pair(p.res2, row * p.ld2 + ocol, in1, a, b);
           v0 = __fmaf_rn(p.s2, a, v0);
           v1 = __fmaf_rn(p.s2, b, v1);
         }
         if (p.out_fp32) {
-          float* op = reinterpret_cast<float*>(p.out) + row[h] * p.ldo + ocol;
-          if (in1 && ((row[h] * p.ldo + ocol) & 1) == 0) {
+          float* op = reinterpret_cast<float*>(p.out) + row * p.ldo + ocol;
+          if (in1 && ((row * p.ldo + ocol) & 1) == 0) {
             *reinterpret_cast<float2*>(op) = make_float2(v0, v1);
           } else {
             op[0] = v0;
             if (in1) op[1] = v1;
           }
         } else {
-          __nv_bfloat16* op = reinterpret_cast<__nv_bfloat16*>(p.out) + row[h] * p.ldo + ocol;
+          __nv_bfloat16* op = reinterpret_cast<__nv_bfloat16*>(p.out) + row * p.ldo + ocol;
           if (in1) {
             *reinterpret_cast<uint32_t*>(op) = pack_bf16x2(v0, v1);  // ldo % 8 == 0 and an even column: 4-byte aligned
           } else {
@@ -965,7 +865,7 @@ mtgemm_alt_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   const int wl = warp & 3;  // warp of the warpgroup: rows 16 wl .. 16 wl + 15 of both 64-row halves
   const int rq = lane >> 2, cq = lane & 3;
   const bool leader = (threadIdx.x & 127) == 0;
-  const uint32_t lb1 = p.m_lb[0], lb2 = p.m_lb[1];
+  const uint32_t rbase = (uint32_t)(16 * wl + rq);
   const uint32_t nres = (p.res1 != nullptr ? 1u : 0u) + (p.res2 != nullptr ? 1u : 0u);
   RingPos ab = {0, 0};   // A/B ring position
   RingPos rr = {0, 0};   // residual ring position
@@ -1026,143 +926,31 @@ mtgemm_alt_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     // ----- epilogue: thread holds rows 64 hh + 16 wl + rq + 8 h, columns 8 j + 2 cq + {0, 1} (accHH[4 j + 2 h + e])
     uint32_t n_tile, mb1, mb2, mb3;
     decode_tile(p, tile, n_tile, mb1, mb2, mb3);
-    const uint32_t n0 = n_tile * BN;
-    const uint32_t otile0 = n_tile * tile_out_w;
-    const float* fv[2][2];
-#pragma unroll
-    for (int hh = 0; hh < 2; ++hh) {
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const uint32_t r = (uint32_t)(64 * hh + 16 * wl + rq + 8 * h);
-        const uint32_t m1 = mb1 + (r & ((1u << lb1) - 1));
-        const uint32_t m2 = mb2 + ((r >> lb1) & ((1u << lb2) - 1));
-        const uint32_t m3 = mb3 + (r >> (lb1 + lb2));
-        const bool valid = (m1 < p.m_ext[0]) && (m2 < p.m_ext[1]) && (m3 < p.m_ext[2]);
-        const int64_t row = (int64_t)m1 * p.out_rs[0] + (int64_t)m2 * p.out_rs[1] + (int64_t)m3 * p.out_rs[2];
-        fv[hh][h] = (p.fvec != nullptr && valid) ? p.fvec + (int64_t)((uint32_t)row / p.rows_per_frame) * p.ldf
-                                                 : nullptr;
-      }
-    }
-    constexpr int NJ = BN / 8;
+    const EpiTile et = {n_tile * BN, n_tile * tile_out_w, n_out, mb1, mb2, mb3, tile / p.n_tiles};
+    const OutRow rows[2][2] = {{out_row(p, et, rbase), out_row(p, et, rbase + 8)},
+                               {out_row(p, et, 64 + rbase), out_row(p, et, 64 + rbase + 8)}};
     if (rslots != 0) {
       pc.mark(PC_EPI);
       while (ld_acquire_shared(&tiles_done[2 + 1 - cw]) < t) {  // ... and tile t - 1's residual slots
       }
       pc.mark(PC_RES_WAIT);
     }
-    if (BN <= 128 && p.epi_kind != B200SVD_EPI_GENERIC) {
-      // ----- epilogue kind known at compile time (launch-uniform: one switch per tile).  Not at BN = 160, whose 160
-      // accumulator registers leave the batched loads no room: that tile keeps the generic body -----
-      const EpiTile et = {n0, otile0, n_out, mb1, mb2, mb3};
-      const float* fvk[2][2];
-#pragma unroll
-      for (int hh = 0; hh < 2; ++hh)
-#pragma unroll
-        for (int h = 0; h < 2; ++h) fvk[hh][h] = fv[hh][h] != nullptr ? fv[hh][h] : p.fvec;
-      const uint32_t rbase = (uint32_t)(16 * wl + rq);
-      switch (p.epi_kind) {
+    // the epilogue kind is launch-uniform: one switch per tile
+    float* const accs[2] = {acc0, acc1};
+    switch (p.epi_kind) {
+      case B200SVD_EPI_GENERIC:
+        epilogue_staged<BN, EpiGeneric, 2>(p, &tmO, et, accs, rows, stg_smem, res_smem, res_full, res_empty, rr,
+                                           stg_it, cw, rbase, cq, leader, nullptr, pc);
+        break;
 #define MTGEMM_CASE(ID, ACT, BIAS, FVEC, NRES)                                                                    \
   case ID:                                                                                                        \
-    if constexpr (BN <= 128 && (ACT != B200SVD_ACT_GEGLU || BN == 128))                                           \
-      alt_epilogue_kind<BN, Epi<ACT, BIAS, FVEC, NRES>>(p, &tmO, et, acc0, acc1, stg_smem, res_smem, res_full,    \
-                                                        res_empty, rslots, rr, stg_it, cw, rbase, (uint32_t)cq,   \
-                                                        leader, fvk, pc);                                         \
+    if constexpr (ACT != B200SVD_ACT_GEGLU || BN == 128)                                                          \
+      epilogue_staged<BN, Epi<ACT, BIAS, FVEC, NRES>, 2>(p, &tmO, et, accs, rows, stg_smem, res_smem, res_full,   \
+                                                         res_empty, rr, stg_it, cw, rbase, cq, leader, nullptr,   \
+                                                         pc);                                                     \
     break;
-        MTGEMM_EPI_KINDS(MTGEMM_CASE)
+      MTGEMM_EPI_KINDS(MTGEMM_CASE)
 #undef MTGEMM_CASE
-      }
-      if (leader && rslots != 0) st_release_shared(&tiles_done[2 + cw], t + 1);
-      continue;
-    }
-#pragma unroll
-    for (int c = 0; c < Cfg::SUBTILES; ++c) {
-      if (geglu && c >= Cfg::SUBTILES / 2) break;  // gate columns are consumed with their value columns
-      if (otile0 + (uint32_t)(c * SUB_W) >= n_out) break;
-      uint8_t* stg = stg_smem + (cw * STG_SLOTS + (stg_it & 1)) * ALT_STG_SLOT_BYTES;
-      // residual sub-tiles (all 128 rows), in the order the residual producer loads them
-      const uint8_t* r1s = nullptr;
-      const uint8_t* r2s = nullptr;
-      uint32_t r1slot = 0, r2slot = 0;
-      pc.mark(PC_EPI);
-      if (p.res1 != nullptr) {
-        r1slot = rr.idx;
-        mbar_wait(&res_full[rr.idx], rr.phase);
-        r1s = res_smem + rr.idx * RES_SLOT_BYTES;
-        ring_step(rr, rslots);
-      }
-      if (p.res2 != nullptr) {
-        r2slot = rr.idx;
-        mbar_wait(&res_full[rr.idx], rr.phase);
-        r2s = res_smem + rr.idx * RES_SLOT_BYTES;
-        ring_step(rr, rslots);
-      }
-      pc.mark(PC_RES_WAIT);
-#pragma unroll
-      for (int jj = 0; jj < 4; ++jj) {
-        const int j = 4 * c + jj;
-        const uint32_t tcol = (uint32_t)(8 * j + 2 * cq);
-        const uint32_t ocol = otile0 + tcol;
-        const bool in0 = ocol < n_out, in1 = ocol + 1 < n_out;
-        float bv[2], gbv[2];
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const bool in = e == 0 ? in0 : in1;
-          bv[e] = (p.bias != nullptr && in) ? __ldg(p.bias + n0 + tcol + e) : 0.f;
-          gbv[e] = (geglu && p.bias != nullptr) ? __ldg(p.bias + n0 + BN / 2 + tcol + e) : 0.f;
-        }
-#pragma unroll
-        for (int hh = 0; hh < 2; ++hh) {
-          float(&acc)[R] = hh == 0 ? acc0 : acc1;
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            const uint32_t off = sw64_off((uint32_t)(64 * hh + 16 * wl + rq + 8 * h), (uint32_t)jj, (uint32_t)cq);
-            float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
-            float g0 = 0.f, g1 = 0.f;
-            if (p.bias != nullptr) {
-              v0 += bv[0];
-              v1 += bv[1];
-            }
-            if (fv[hh][h] != nullptr) {
-              v0 += in0 ? __ldg(fv[hh][h] + ocol) : 0.f;
-              v1 += in1 ? __ldg(fv[hh][h] + ocol + 1) : 0.f;
-            }
-            if (geglu) {
-              g0 = acc[4 * (j + NJ / 2) + 2 * h];
-              g1 = acc[4 * (j + NJ / 2) + 2 * h + 1];
-              if (p.bias != nullptr) {
-                g0 += gbv[0];
-                g1 += gbv[1];
-              }
-            }
-            v0 = epi_act(p, geglu, v0, g0);
-            v1 = epi_act(p, geglu, v1, g1);
-            if (r1s != nullptr) {
-              const uint32_t w = *reinterpret_cast<const uint32_t*>(r1s + off);
-              v0 = __fmaf_rn(p.s1, bf16_lo(w), v0);
-              v1 = __fmaf_rn(p.s1, bf16_hi(w), v1);
-            }
-            if (r2s != nullptr) {
-              const uint32_t w = *reinterpret_cast<const uint32_t*>(r2s + off);
-              v0 = __fmaf_rn(p.s2, bf16_lo(w), v0);
-              v1 = __fmaf_rn(p.s2, bf16_hi(w), v1);
-            }
-            *reinterpret_cast<uint32_t*>(stg + off) = pack_bf16x2(v0, v1);
-          }
-        }
-      }
-      fence_proxy_async_smem();  // the staged values are read by the TMA store (async proxy)
-      pc.mark(PC_EPI);
-      // the store issued one sub-tile ago has read the other staging buffer: it may be refilled next sub-tile
-      if (leader) tma_store_wait_read0();
-      named_bar_sync(5 + (int)cw, 128);
-      pc.mark(PC_STORE_WAIT);
-      if (leader) {
-        if (r1s != nullptr) mbar_arrive(&res_empty[r1slot]);
-        if (r2s != nullptr) mbar_arrive(&res_empty[r2slot]);
-        tma_store_4d(&tmO, stg, (int)(otile0 + c * SUB_W), (int)mb1, (int)mb2, (int)mb3);  // the tile's row box
-        tma_store_commit();
-      }
-      ++stg_it;
     }
     if (leader && rslots != 0) st_release_shared(&tiles_done[2 + cw], t + 1);
   }
@@ -1262,10 +1050,12 @@ static int g_schedule = 2;
 constexpr uint64_t ALT_MAX_TILE_MMA_CLOCKS = 20000;
 
 // N tile of the alternating schedule for a launch whose cooperative tile is `bn`, 0 if it has none.  A GEGLU launch
-// cannot change its tile: the weights are interleaved per tile.
+// cannot change its tile: the weights are interleaved per tile.  The 160-wide tile (N = 160, 320) has none: it
+// measured slower alternating than cooperative (M 460800, K 1280, N 320 with a residual: 3.2 ms against 1.4 ms on an
+// H100 at 700 W), and its 160 accumulator registers per thread leave the batched epilogue loads no room.
 static int alt_tile(int bn, bool geglu) {
   if (bn == 256 && !geglu) return 128;
-  return bn <= 160 ? bn : 0;
+  return bn <= 128 ? bn : 0;
 }
 
 // Epilogue body choice, see b200svd_gemm_epilogue in b200svd.h.
@@ -1453,11 +1243,6 @@ extern "C" int b200svd_gemm(const b200svd_gemm_params* p, void* stream) {
   if (d.staged && p->gn_part == nullptr && g_schedule != 0) {
     alt_bn = alt_tile(bn, p->act == B200SVD_ACT_GEGLU);
     if (alt_bn != 0 && g_schedule == 2) {
-      // The 160-wide tile (N = 160, 320) measured slower alternating than cooperative (M 460800, K 1280, N 320 with a
-      // residual: 3.2 ms against 1.4 ms on an H100 at 700 W), so the rule leaves it cooperative; mode 1 still runs it.
-      if (alt_bn == 160) alt_bn = 0;
-    }
-    if (alt_bn != 0 && g_schedule == 2) {
       const uint64_t tiles = m_tiles_all * ((p->n + alt_bn - 1) / alt_bn);
       const uint64_t mma_clocks = (uint64_t)d.taps * d.kblocks * 2 * alt_bn;
       if (tiles < 2 * (uint64_t)sm_count() || mma_clocks >= ALT_MAX_TILE_MMA_CLOCKS) alt_bn = 0;
@@ -1504,7 +1289,6 @@ extern "C" int b200svd_gemm(const b200svd_gemm_params* p, void* stream) {
     case 32: return launch<32, true>(p, tmA, em, d, st);
     case 64: return launch<64, true>(p, tmA, em, d, st);
     case 128: return launch<128, true>(p, tmA, em, d, st);
-    case 160: return launch<160, true>(p, tmA, em, d, st);
   }
   switch (bn) {
     case 32: return launch<32>(p, tmA, em, d, st);

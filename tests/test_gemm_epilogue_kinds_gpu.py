@@ -1,10 +1,11 @@
 """The compile-time epilogue kinds of the wgmma GEMM against the generic epilogue body: bitwise the same output.
 
 Every specialised kind runs on both schedules at the N tiles 64, 128, 160 and 256 (GEGLU at 128 and 256, the tiles
-its weights can be packed for), with rows that do not fill the last M tile and, except for GEGLU, a ragged last N
-tile, once with gemm_epilogue(0) and once with gemm_epilogue(1) into NaN-filled guard buffers.  The outputs must be
-equal bit for bit, fully written, and nothing outside the output view may change.  One profiled forward of the small
-denoiser must have no staged bf16 launch that falls back to the generic body.
+its weights can be packed for; the 160-wide tile has no alternating form and runs cooperative on both), with rows
+that do not fill the last M tile and, except for GEGLU, a ragged last N tile, once with gemm_epilogue(0) and once
+with gemm_epilogue(1) into NaN-filled guard buffers.  The outputs must be equal bit for bit, fully written, and
+nothing outside the output view may change.  One profiled forward of the small denoiser must have no staged bf16
+launch that falls back to the generic body.
 """
 import ctypes as C
 
