@@ -26,7 +26,7 @@ extern "C" {
 
 #define B200SVD_MAX_TAPS 12
 
-enum { B200SVD_ACT_NONE = 0, B200SVD_ACT_SILU = 1, B200SVD_ACT_GELU = 2, B200SVD_ACT_GEGLU = 3 };
+enum { B200SVD_ACT_NONE = 0, B200SVD_ACT_SILU = 1, B200SVD_ACT_GELU = 2, B200SVD_ACT_GEGLU = 3, B200SVD_ACT_PRELU = 4 };
 
 /* ---- library ------------------------------------------------------------------------------------------- */
 const char* b200svd_last_error(void);
@@ -90,6 +90,11 @@ typedef struct {
   int32_t* gn_slot_sample;
   int64_t gn_ld;     /* channels per slot row of gn_part (>= n) */
   uint32_t gn_rows;  /* output rows per GroupNorm sample */
+  /* act = B200SVD_ACT_PRELU: nn.PReLU with one slope per output column (EMA-VFI conv + PReLU, VFI/model/refine.py:8-19,
+   * feature_extractor.py:283-295), v > 0 ? v : slope[n] * v, applied where the other activations are.  fp32 [n];
+   * required with PReLU, ignored otherwise.  PReLU outputs are stored straight from the accumulator registers (the
+   * path of fp32 outputs), never staged. */
+  const float* slope;
 } b200svd_gemm_params;
 
 int b200svd_gemm(const b200svd_gemm_params* p, void* stream);
@@ -279,6 +284,53 @@ int b200svd_frames_to_uint8(const float* x, void* out, int64_t n, int c, int64_t
  * The result lies on the 1/127.5 grid; unlike b200svd_frames_to_uint8 (which truncates, as torch2np does) it rounds.
  * out may alias x. */
 int b200svd_frames_quantize(const float* x, float* out, int64_t n, void* stream);
+
+/* ---- EMA-VFI frame interpolation (the interpolate stage: i2v_enhance_interface.vfi_process, thirdparty/VFI) ---------
+ * vfi_window_attn: InterFrameAttention of MotionFormerBlock (feature_extractor.py:146-172, 213-277) on 7x7 windows,
+ *   head dim 32, motion dim 8 per head, with the centre padding to multiples of 7, the shift roll (shift 0 or 3), the
+ *   -100 shift / padding masks and the pairing of image b with image (b + pairs) mod 2*pairs done by addressing.
+ *   qkv: bf16 rows [2*pairs*h*w + 1][ldq], image-major, columns [q | k | v] each heads*32 wide; the last row is the
+ *   padding token (the projections of LayerNorm(0)).  cor_embed: bf16 [h*w + 1][ldc], heads*8 columns, the last row
+ *   the padding token.  Writes, for every real token, out = attn @ v (heads*32 columns) and motion =
+ *   attn @ cor_embed - cor_embed (heads*8 columns).  Errors: qkv / cor_embed not 16-byte aligned or leading dims not
+ *   multiples of 8.
+ * vfi_warp: warplayer.warp, grid_sample(bilinear, padding border, align_corners=True) at linspace grid + flow /
+ *   ((size-1)/2).  Elements (n, c, y, x) of in / flow / out at the given element strides; flow points at its x channel
+ *   (y channel one channel stride further).  in fp32 or bf16, out fp32 or bf16 (bf16 in needs bf16 out); h, w >= 2.
+ * vfi_resize: F.interpolate(bilinear, align_corners=False, scale_factor = 2^factor_log2, factor_log2 in
+ *   {-2, -1, 1, 2}) of fp32 in [n][c][h][w] (element strides), times mul, written (fp32 or bf16) or, with accumulate
+ *   (fp32 only), added to out.
+ * vfi_dwconv_gelu: depthwise 3x3 conv (zero pad 1) + bias + exact GELU, bf16 [n][h][w][c] -> [n][h][w][c], weights
+ *   fp32 [9][c] (tap kh*3+kw); c % 8 == 0, 16-byte aligned x and y.
+ * vfi_head_gather: Head input (flow_estimation.py:28-29, 81-89) at timestep 0.5: PixelShuffle(2) twice of
+ *   cat([0.5 mf[:pairs], 0.5 mf[pairs:], af[:pairs], af[pairs:]]) with mf, af bf16 rows [2*pairs*h*w][ld] of c
+ *   channels -> out bf16 rows [pairs*4h*4w][ldo], columns 0..c/4-1.
+ * vfi_merge: the last stage of the fast-TTA prediction (flow_estimation.py:133-140, Trainer.py:95-99): per copy b of
+ *   the TTA pair, clamp(w0 sigmoid(mask) + w1 (1 - sigmoid(mask)) + 2 sigmoid(res) - 1, 0, 1), copy 1 mirrored, the
+ *   two averaged.  warped0/1 fp32 [2][3][h][w], fm fp32 [2][5][h][w] (mask = channel 4), res fp32 rows [2*h*w][ldr]
+ *   (3 columns, pre-sigmoid).  pred (optional) fp32 [3][h][w] BGR; frame (optional) uint8 [h][w][3] RGB =
+ *   uint8(pred * 255) truncating (vfi_process, i2v_enhance_interface.py:46-48).
+ * vfi_pair_input: imgs fp32 [4][3][h][w] = [img0, flip(img0), img1, flip(img1)] from img0 / img1 fp32 [3][h][w], and
+ *   the same as bf16 [4][h][w][8] with channels 3..7 zero (16-byte aligned).
+ * vfi_frames_to_bgr: uint8 RGB [n][h][w][3] -> fp32 BGR [n][3][h][w], (float)(u / 255.0) (i2v_enhance_interface.py:33-37).
+ * Every entry point launches nothing and returns 0 when its output has no elements. */
+int b200svd_vfi_window_attn(const void* qkv, int64_t ldq, const void* cor_embed, int64_t ldc, void* out, int64_t ldo,
+                            void* motion, int64_t ldm, int pairs, int h, int w, int heads, int shift, float scale,
+                            void* stream);
+int b200svd_vfi_warp(const void* in, int in_bf16, int64_t isn, int64_t isc, int64_t isy, int64_t isx,
+                     const float* flow, int64_t fsn, int64_t fsc, int64_t fsy, int64_t fsx, void* out, int out_bf16,
+                     int64_t osn, int64_t osc, int64_t osy, int64_t osx, int n, int c, int h, int w, void* stream);
+int b200svd_vfi_resize(const float* in, int64_t isn, int64_t isc, int64_t isy, int64_t isx, void* out, int out_bf16,
+                       int64_t osn, int64_t osc, int64_t osy, int64_t osx, int n, int c, int h, int w, int factor_log2,
+                       float mul, int accumulate, void* stream);
+int b200svd_vfi_dwconv_gelu(const void* x, void* y, int n, int h, int w, int c, const float* wt, const float* bias,
+                            void* stream);
+int b200svd_vfi_head_gather(const void* mf, int64_t ldm, const void* af, int64_t lda, int pairs, int h, int w, int c,
+                            void* out, int64_t ldo, void* stream);
+int b200svd_vfi_merge(const float* warped0, const float* warped1, const float* fm, const float* res, int64_t ldr,
+                      int h, int w, float* pred, void* frame, void* stream);
+int b200svd_vfi_pair_input(const float* img0, const float* img1, int h, int w, float* imgs, void* x8, void* stream);
+int b200svd_vfi_frames_to_bgr(const void* frames, int64_t n, int h, int w, float* out, void* stream);
 
 #ifdef __cplusplus
 }

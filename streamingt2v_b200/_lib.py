@@ -14,7 +14,7 @@ _LIB = None
 LIB_PATH = Path(__file__).resolve().parent / "libb200svd.so"
 
 MAX_TAPS = 12
-ACT_NONE, ACT_SILU, ACT_GELU, ACT_GEGLU = 0, 1, 2, 3
+ACT_NONE, ACT_SILU, ACT_GELU, ACT_GEGLU, ACT_PRELU = 0, 1, 2, 3, 4
 # B200SVD_EPI_*: compile-time epilogue kinds of the GEMM, 0 = the generic body
 (EPI_GENERIC, EPI_PLAIN, EPI_BIAS, EPI_BIAS_RES1, EPI_BIAS_RES1_FVEC, EPI_BIAS_FVEC, EPI_BIAS_GEGLU, EPI_BIAS_RES2,
  EPI_BIAS_SILU, EPI_BIAS_GELU) = range(10)
@@ -55,6 +55,7 @@ class GemmParams(C.Structure):
         ("gn_slot_sample", C.c_void_p),
         ("gn_ld", C.c_int64),
         ("gn_rows", C.c_uint32),
+        ("slope", C.c_void_p),
     ]
 
 
@@ -124,6 +125,15 @@ PROTOTYPES = {
     "b200svd_frames_to_uint8": [_P, _P, _I64, _I, _I64, _F, _F, _P],
     "b200svd_frames_quantize": [_P, _P, _I64, _P],
     "b200svd_ddim_blend_step": [_P, _P, _P, _I, _I, _I64, _I, _I, _I, _I, _I, _I, _F, _F, _F, _I, _P],
+    "b200svd_vfi_window_attn": [_P, _I64, _P, _I64, _P, _I64, _P, _I64, _I, _I, _I, _I, _I, _F, _P],
+    "b200svd_vfi_warp": [_P, _I, _I64, _I64, _I64, _I64, _P, _I64, _I64, _I64, _I64, _P, _I, _I64, _I64, _I64, _I64,
+                         _I, _I, _I, _I, _P],
+    "b200svd_vfi_resize": [_P, _I64, _I64, _I64, _I64, _P, _I, _I64, _I64, _I64, _I64, _I, _I, _I, _I, _I, _F, _I, _P],
+    "b200svd_vfi_dwconv_gelu": [_P, _P, _I, _I, _I, _I, _P, _P, _P],
+    "b200svd_vfi_head_gather": [_P, _I64, _P, _I64, _I, _I, _I, _I, _P, _I64, _P],
+    "b200svd_vfi_merge": [_P, _P, _P, _P, _I64, _I, _I, _P, _P, _P],
+    "b200svd_vfi_pair_input": [_P, _P, _I, _I, _P, _P, _P],
+    "b200svd_vfi_frames_to_bgr": [_P, _I64, _I, _I, _P, _P],
 }
 
 

@@ -71,6 +71,7 @@ struct GemmDev {
   uint32_t stages;     // depth of the A/B stage ring
   uint32_t res_slots;  // depth of the residual ring (bf16 outputs with residuals, else 0)
   uint32_t wg_off[3];  // row-box origin of the second consumer warpgroup's 64 rows (bf16 output stores)
+  const float* slope;  // PReLU slope per GEMM column (act = B200SVD_ACT_PRELU)
 #ifdef MTGEMM_PHASE_CLOCKS
   long long* phase_buf;  // [CTA][role][PC_N] clock sums, see PhaseClock
 #endif
@@ -220,7 +221,8 @@ __device__ __forceinline__ void load_bf16_pair(const __nv_bfloat16* base, int64_
 }
 
 // The epilogue arithmetic after bias and per-frame vector, shared by the fp32 and the bf16 output paths so that both
-// round the same fp32 value: activation (GEGLU: value * GELU(gate + gate bias), the gate bias already added), scale.
+// round the same fp32 value: activation (GEGLU: value * GELU(gate + gate bias), the gate bias already added; PReLU: g is
+// the column's slope), scale.
 // Multiplies and fused multiply-adds are written out so that the compiler cannot contract them differently.  An
 // activation known at compile time folds the tests away.
 __device__ __forceinline__ float epi_act(int act, float s_acc, float v, float g) {
@@ -230,6 +232,8 @@ __device__ __forceinline__ float epi_act(int act, float s_acc, float v, float g)
     v = gelu_fast(v);
   } else if (act == B200SVD_ACT_GEGLU) {
     v = __fmul_rn(v, gelu_fast(g));
+  } else if (act == B200SVD_ACT_PRELU) {
+    v = v > 0.f ? v : __fmul_rn(g, v);
   }
   return __fmul_rn(v, s_acc);
 }
@@ -752,6 +756,9 @@ mtgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
             g0 += __ldg(p.bias + et.n0 + BN / 2 + tcol);
             if (in1) g1 += __ldg(p.bias + et.n0 + BN / 2 + tcol + 1);
           }
+        } else if (p.act == B200SVD_ACT_PRELU) {
+          g0 = __ldg(p.slope + et.n0 + tcol);
+          if (in1) g1 = __ldg(p.slope + et.n0 + tcol + 1);
         }
         v0 = epi_act(p.act, p.s_acc, v0, g0);
         v1 = epi_act(p.act, p.s_acc, v1, g1);
@@ -1189,6 +1196,11 @@ extern "C" int b200svd_gemm(const b200svd_gemm_params* p, void* stream) {
   d.gn_slot_sample = p->gn_slot_sample;
   d.gn_ld = p->gn_ld;
   d.gn_rows = p->gn_rows ? p->gn_rows : 1;
+  if (p->act < B200SVD_ACT_NONE || p->act > B200SVD_ACT_PRELU || (p->act == B200SVD_ACT_PRELU && p->slope == nullptr)) {
+    set_error("b200svd_gemm: act=%d is not a B200SVD_ACT_* value, or PReLU without slopes", (int)p->act);
+    return 1;
+  }
+  d.slope = p->slope;
 
   int bn = p->bn;
   if (p->act == B200SVD_ACT_GEGLU) {
@@ -1237,7 +1249,9 @@ extern "C" int b200svd_gemm(const b200svd_gemm_params* p, void* stream) {
   // store writes whole 16-byte chunks of a row, so this needs an output width that is a multiple of 8.
   EpiMaps em;
   memset(&em, 0, sizeof(em));
-  d.staged = !p->out_fp32 && n_out % 8 == 0;
+  // PReLU stores from registers: its per-column slopes in the staged body would cost the cooperative 128-wide kernel
+  // registers it does not have (ptxas spills), and no other launch uses them.
+  d.staged = !p->out_fp32 && n_out % 8 == 0 && p->act != B200SVD_ACT_PRELU;
   d.epi_kind = g_epilogue != 0 ? epilogue_kind(p) : B200SVD_EPI_GENERIC;
   int alt_bn = 0;
   if (d.staged && p->gn_part == nullptr && g_schedule != 0) {

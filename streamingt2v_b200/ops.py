@@ -13,7 +13,7 @@ from functools import lru_cache
 import torch
 
 from . import _lib
-from ._lib import ACT_GEGLU, ACT_GELU, ACT_NONE, ACT_SILU, GemmParams
+from ._lib import ACT_GEGLU, ACT_GELU, ACT_NONE, ACT_PRELU, ACT_SILU, GemmParams
 
 _launch_count = 0
 _PROFILE = None  # list of (family, flops, bytes, start_event, end_event) while profiling
@@ -137,7 +137,7 @@ def pick_box(e1: int, e2: int, e3: int):
 
 def gemm_raw(*, a, a_dims, a_strides, a_box, w, n, k, taps, tap_off, m_ext, m_box, m_adim, out, ldo, out_rs=None,
              out_fp32=False, bias=None, fvec=None, ldf=0, rows_per_frame=1, act=ACT_NONE, s_acc=1.0, res1=None,
-             ld1=0, s1=1.0, res2=None, ld2=0, s2=1.0, bn=0, gn=None):
+             ld1=0, s1=1.0, res2=None, ld2=0, s2=1.0, bn=0, gn=None, slope=None):
     global _launch_count
     p = GemmParams()
     p.a_ptr = a.data_ptr()
@@ -174,6 +174,9 @@ def gemm_raw(*, a, a_dims, a_strides, a_box, w, n, k, taps, tap_off, m_ext, m_bo
     p.ld2 = int(ld2)
     p.s2 = float(s2)
     p.bn = int(bn)
+    if slope is not None:
+        assert slope.dtype == torch.float32 and slope.is_contiguous() and slope.numel() >= n
+        p.slope = slope.data_ptr()
     if gn is not None:
         p.gn_part = gn["part"].data_ptr()
         p.gn_slot_sample = gn["slot"].data_ptr()
@@ -237,8 +240,11 @@ def _gn_request(gn_rows, m_ext, m_box, n_out, act, out_fp32, device):
                 C=int(n_out))
 
 
-def _epi_kwargs(rows, n_out, out, bias, fvec, rows_per_frame, act, s_acc, res1, s1, res2, s2, out_fp32):
+def _epi_kwargs(rows, n_out, out, bias, fvec, rows_per_frame, act, s_acc, res1, s1, res2, s2, out_fp32, slope=None):
     kw = dict(bias=bias, act=act, s_acc=s_acc, out_fp32=out_fp32)
+    assert (act == ACT_PRELU) == (slope is not None), "PReLU takes a slope vector, nothing else does"
+    if slope is not None:
+        kw.update(slope=slope)
     if fvec is not None:
         assert fvec.dtype == torch.float32 and fvec.stride(-1) == 1
         kw.update(fvec=fvec, ldf=fvec.stride(0), rows_per_frame=rows_per_frame)
@@ -259,7 +265,7 @@ def _alloc_out(rows, n_out, out, out_fp32, device):
 
 
 def linear(x, w, bias=None, *, act=ACT_NONE, out=None, out_fp32=False, fvec=None, rows_per_frame=1, s_acc=1.0,
-           res1=None, s1=1.0, res2=None, s2=1.0, bn=0, gn_rows=None):
+           res1=None, s1=1.0, res2=None, s2=1.0, bn=0, gn_rows=None, slope=None):
     """x: [M, K] bf16 (row stride arbitrary, multiple of 8); w: packed [1, N, K] bf16; returns [M, N_out]."""
     assert x.dtype == torch.bfloat16 and x.dim() == 2 and x.stride(1) == 1
     M, K = x.shape
@@ -273,7 +279,7 @@ def linear(x, w, bias=None, *, act=ACT_NONE, out=None, out_fp32=False, fvec=None
     gemm_raw(a=x, a_dims=(K, M, 1, 1, 1), a_strides=(ld * 2, big, big, big), a_box=(64, 128, 1, 1, 1),
              w=w, n=N, k=K, taps=1, tap_off=[(0, 0, 0, 0, 0)], m_ext=(M, 1, 1), m_box=(128, 1, 1),
              m_adim=(1, 2, 3), out=out, ldo=out.stride(0), bn=bn, gn=gn,
-             **_epi_kwargs(M, n_out, out, bias, fvec, rows_per_frame, act, s_acc, res1, s1, res2, s2, out_fp32))
+             **_epi_kwargs(M, n_out, out, bias, fvec, rows_per_frame, act, s_acc, res1, s1, res2, s2, out_fp32, slope))
     if gn is not None:
         out._b200_gn = gn          # consumed by group_norm(out, ...) instead of a statistics pass over `out`
     return out
@@ -331,7 +337,7 @@ def tconv3(x, w, bias=None, *, out=None, **epi):
                         (64, b1, b2, b3, 1), w, Cout, Cc, taps, (P, T, B), (b1, b2, b3), (1, 2, 3), bias, out, epi)
 
 
-def _conv_common(x, a_dims, a_strides, a_box, w, Cout, K, taps, m_ext, m_box, m_adim, bias, out, epi):
+def _conv_common(x, a_dims, a_strides, a_box, w, Cout, K, taps, m_ext, m_box, m_adim, bias, out, epi, out_rs=None):
     rows = m_ext[0] * m_ext[1] * m_ext[2]
     act = epi.pop("act", ACT_NONE)
     out_fp32 = epi.pop("out_fp32", False)
@@ -340,11 +346,11 @@ def _conv_common(x, a_dims, a_strides, a_box, w, Cout, K, taps, m_ext, m_box, m_
     out = _alloc_out(rows, n_out, out, out_fp32, x.device)
     kw = _epi_kwargs(rows, n_out, out, bias, epi.pop("fvec", None), epi.pop("rows_per_frame", 1), act,
                      epi.pop("s_acc", 1.0), epi.pop("res1", None), epi.pop("s1", 1.0), epi.pop("res2", None),
-                     epi.pop("s2", 1.0), out_fp32)
+                     epi.pop("s2", 1.0), out_fp32, epi.pop("slope", None))
     gn = _gn_request(epi.pop("gn_rows", None), m_ext, m_box, n_out, act, out_fp32, x.device)
     assert not epi, f"unknown epilogue args {list(epi)}"
     gemm_raw(a=x, a_dims=a_dims, a_strides=a_strides, a_box=a_box, w=w, n=Cout, k=K, taps=len(taps), tap_off=taps,
-             m_ext=m_ext, m_box=m_box, m_adim=m_adim, out=out, ldo=out.stride(0), bn=bn, gn=gn, **kw)
+             m_ext=m_ext, m_box=m_box, m_adim=m_adim, out=out, ldo=out.stride(0), out_rs=out_rs, bn=bn, gn=gn, **kw)
     if gn is not None:
         out._b200_gn = gn
     return out
@@ -692,4 +698,177 @@ def attention_single_head(q, k, v, n, s):
         probs = softmax_rows(scores)
         vt = transpose(v[sl])                                                           # [C, s]
         linear(probs, vt[None], None, out=out[sl])
+    return out
+
+
+# ----------------------------------------------------------------------------------------------------------------
+# EMA-VFI frame interpolation (csrc/vfi.cu)
+# ----------------------------------------------------------------------------------------------------------------
+_FAMILY.update({"b200svd_vfi_window_attn": "vfi_attn", "b200svd_vfi_warp": "vfi_warp", "b200svd_vfi_resize": "vfi_resize",
+                "b200svd_vfi_dwconv_gelu": "vfi_dwconv", "b200svd_vfi_head_gather": "glue", "b200svd_vfi_merge": "glue",
+                "b200svd_vfi_pair_input": "glue", "b200svd_vfi_frames_to_bgr": "glue"})
+
+
+def conv3x3_strided(x, w, bias=None, *, stride, dilation, out=None, **epi):
+    """3x3 conv with stride s in {2, 4, 8} and padding = dilation = d < s (CrossScalePatchEmbed,
+    feature_extractor.py:352-354).  x: [N, H, W, C] bf16 contiguous, H and W multiples of s.  The input is viewed as
+    [N, H/s, s, W/s, s*C]; input row s*i + d*(k-1) is output row i + q at phase r (s*q + r = d*(k-1)), so every tap
+    is a shifted TMA box and the rows above / left of the image (q = -1) are the zero padding."""
+    assert x.dtype == torch.bfloat16 and x.dim() == 4 and x.is_contiguous()
+    N, H, W, Cc = x.shape
+    s, d = int(stride), int(dilation)
+    assert s in (2, 4, 8) and 1 <= d < s and H % s == 0 and W % s == 0
+    Ho, Wo = H // s, W // s
+    Cout = w.shape[1]
+    assert w.shape == (9, Cout, Cc) and w.is_contiguous()
+    b1, b2, b3 = pick_box(Wo, Ho, N)
+    taps = []
+    for kh in range(3):
+        qh, rh = divmod(d * (kh - 1), s)
+        for kw in range(3):
+            qw, rw = divmod(d * (kw - 1), s)
+            taps.append((rw * Cc, qw, rh, qh, 0))
+    return _conv_common(x, (s * Cc, Wo, s, Ho, N),
+                        (s * Cc * 2, W * Cc * 2, s * W * Cc * 2, H * W * Cc * 2),
+                        (64, b1, 1, b2, b3), w, Cout, Cc, taps, (Wo, Ho, N), (b1, b2, b3), (1, 3, 4), bias, out, epi)
+
+
+# ConvTranspose2d(4, stride 2, padding 1): output row 2i + a takes input rows i - 1 (kernel row 3) and i (1) for a = 0,
+# i (2) and i + 1 (0) for a = 1; the same along the width.  (offset, kernel index) per output phase.
+DECONV_PHASE_TAPS = (((-1, 3), (0, 1)), ((0, 2), (1, 0)))
+
+
+def conv_transpose4x4_s2(x, w, bias=None, *, out, **epi):
+    """ConvTranspose2d(k=4, s=2, p=1) as one 4-tap GEMM per output phase (a, b): output pixel (2i + a, 2j + b) sums
+    the 2x2 input pixels DECONV_PHASE_TAPS names, so each launch is a stride-1 conv with 4 of the 9 taps and its rows
+    go straight to every other pixel of the 2x output through the GEMM's output row strides.
+    x: [N, H, W, C] bf16 contiguous; w: packed [4 phases (a*2+b), 4 taps, Cout, C]; out: rows [(N 2H 2W), >= Cout]
+    (row stride free).  Returns out."""
+    assert x.dtype == torch.bfloat16 and x.dim() == 4 and x.is_contiguous()
+    N, H, W, Cc = x.shape
+    Cout = w.shape[2]
+    assert w.shape == (4, 4, Cout, Cc) and w.is_contiguous() and out.shape[0] == N * 4 * H * W
+    b1, b2, b3 = pick_box(W, H, N)
+    for a in range(2):
+        for b in range(2):
+            taps = [(0, dx, dy, 0, 0) for dy, _ in DECONV_PHASE_TAPS[a] for dx, _ in DECONV_PHASE_TAPS[b]]
+            _conv_common(x, (Cc, W, H, N, 1), (Cc * 2, W * Cc * 2, H * W * Cc * 2, N * H * W * Cc * 2),
+                         (64, b1, b2, b3, 1), w[a * 2 + b], Cout, Cc, taps, (W, H, N), (b1, b2, b3), (1, 2, 3), bias,
+                         out[a * 2 * W + b:], dict(epi), out_rs=(2, 4 * W, 4 * H * W))
+    return out
+
+
+def vfi_window_attn(qkv, cor_embed, *, pairs, h, w, heads, shift, out, motion):
+    """InterFrameAttention of one MotionFormerBlock over all windows (see b200svd_vfi_window_attn).  qkv: bf16 rows
+    [2*pairs*h*w + 1, >= 3*heads*32] (last row = padding token); cor_embed: bf16 [h*w + 1, >= heads*8]; out: bf16
+    [2*pairs*h*w, >= heads*32]; motion: bf16 [2*pairs*h*w, >= heads*8] (row strides free)."""
+    for t in (qkv, cor_embed, out, motion):
+        assert t.dtype == torch.bfloat16 and t.dim() == 2 and t.stride(1) == 1
+    T = 2 * pairs * h * w
+    assert qkv.shape[0] == T + 1 and cor_embed.shape[0] == h * w + 1 and out.shape[0] == T and motion.shape[0] == T
+    hp, wp = -(-h // 7) * 7, -(-w // 7) * 7
+    blocks = (hp // 7) * (wp // 7) * heads * 2 * pairs
+    _call("b200svd_vfi_window_attn", _ptr(qkv), qkv.stride(0), _ptr(cor_embed), cor_embed.stride(0), _ptr(out),
+          out.stride(0), _ptr(motion), motion.stride(0), pairs, h, w, heads, shift, 32 ** -0.5, _stream(),
+          flops=blocks * 2.0 * 49 * 49 * (32 + 32 + 8), nbytes=blocks * 49 * 2.0 * (3 * 32 + 8 + 32 + 8),
+          desc=f"{h}x{w} h{heads} shift{shift}")
+    return out, motion
+
+
+def _nchw_strides(t):
+    assert t.dim() == 4
+    return [int(v) for v in t.stride()]
+
+
+def vfi_warp(inp, flow, out):
+    """Backward warp (warplayer.warp): out = grid_sample(inp, linspace grid + flow, bilinear, border,
+    align_corners=True).  inp / out: [n, c, h, w] views with any element strides (fp32 or bf16; a bf16 input needs a
+    bf16 output), flow: [n, 2, h, w] fp32 view (x then y)."""
+    n, c, h, w = inp.shape
+    assert out.shape == inp.shape and flow.shape == (n, 2, h, w) and flow.dtype == torch.float32
+    ib, ob = inp.dtype == torch.bfloat16, out.dtype == torch.bfloat16
+    _call("b200svd_vfi_warp", _ptr(inp), int(ib), *_nchw_strides(inp), _ptr(flow), *_nchw_strides(flow), _ptr(out),
+          int(ob), *_nchw_strides(out), n, c, h, w, _stream(),
+          nbytes=n * h * w * (8.0 + c * (4 * (2 if ib else 4) + (2 if ob else 4))), desc=f"{n}x{c}x{h}x{w}")
+    return out
+
+
+def vfi_resize(inp, out, factor_log2, mul=1.0, accumulate=False):
+    """F.interpolate(inp, scale_factor=2**factor_log2, mode="bilinear", align_corners=False) * mul, written to out or,
+    with accumulate, added to it.  inp: fp32 [n, c, h, w] view, out: [n, c, h*f, w*f] view (fp32, or bf16 without
+    accumulate); any element strides."""
+    n, c, h, w = inp.shape
+    assert inp.dtype == torch.float32
+    f = 2.0 ** factor_log2
+    assert out.shape == (n, c, int(h * f), int(w * f))
+    ob = out.dtype == torch.bfloat16
+    _call("b200svd_vfi_resize", _ptr(inp), *_nchw_strides(inp), _ptr(out), int(ob), *_nchw_strides(out), n, c, h, w,
+          int(factor_log2), float(mul), int(accumulate), _stream(),
+          nbytes=out.numel() * (4.0 * (1 + accumulate) + (2 if ob else 4)) + 4.0 * inp.numel(),
+          desc=f"{n}x{c}x{h}x{w} x2^{factor_log2}")
+    return out
+
+
+def vfi_dwconv_gelu(x, wt, bias, out=None):
+    """x: bf16 [N, H, W, C] contiguous; wt: fp32 [9, C] (tap kh*3+kw); bias fp32 [C] -> GELU(dwconv3x3(x) + bias),
+    bf16 rows [(N H W), C]."""
+    assert x.dtype == torch.bfloat16 and x.dim() == 4 and x.is_contiguous()
+    N, H, W, Cc = x.shape
+    assert wt.shape == (9, Cc) and wt.dtype == torch.float32 and wt.is_contiguous() and bias.numel() == Cc
+    if out is None:
+        out = torch.empty((N * H * W, Cc), dtype=torch.bfloat16, device=x.device)
+    assert out.is_contiguous() and out.shape == (N * H * W, Cc)
+    _call("b200svd_vfi_dwconv_gelu", _ptr(x), _ptr(out), N, H, W, Cc, _ptr(wt), _ptr(bias), _stream(),
+          flops=18.0 * x.numel(), nbytes=4.0 * x.numel(), desc=f"{N}x{H}x{W}x{Cc}")
+    return out
+
+
+def vfi_head_gather(mf, af, *, pairs, h, w, out):
+    """Head input at timestep 0.5 (see b200svd_vfi_head_gather): mf, af bf16 rows [2*pairs*h*w, c] -> out bf16 rows
+    [pairs*4h*4w, >= c/4] (columns 0..c/4-1 written)."""
+    c = mf.shape[1]
+    assert af.shape[1] == c and mf.shape[0] == af.shape[0] == 2 * pairs * h * w and out.shape[0] == pairs * 16 * h * w
+    for t in (mf, af, out):
+        assert t.dtype == torch.bfloat16 and t.stride(1) == 1
+    _call("b200svd_vfi_head_gather", _ptr(mf), mf.stride(0), _ptr(af), af.stride(0), pairs, h, w, c, _ptr(out),
+          out.stride(0), _stream(), nbytes=8.0 * mf.numel(), desc=f"{h}x{w} c{c}")
+    return out
+
+
+def vfi_merge(warped0, warped1, fm, res, *, pred=None, frame=None):
+    """Final fast-TTA prediction (see b200svd_vfi_merge): warped0/1 fp32 [2, 3, H, W], fm fp32 [2, 5, H, W] (channel 4
+    = mask logit), res fp32 rows [2*H*W, >= 3] (pre-sigmoid refinement).  Writes pred fp32 [1, 3, H, W] (BGR) and/or
+    frame uint8 [H, W, 3] (RGB)."""
+    _, _, H, W = warped0.shape
+    for t in (warped0, warped1, fm):
+        assert t.dtype == torch.float32 and t.is_contiguous() and t.shape[0] == 2 and t.shape[2:] == (H, W)
+    assert res.dtype == torch.float32 and res.stride(1) == 1 and res.shape[0] == 2 * H * W
+    assert pred is None or (pred.dtype == torch.float32 and pred.is_contiguous() and pred.numel() == 3 * H * W)
+    assert frame is None or (frame.dtype == torch.uint8 and frame.is_contiguous() and frame.shape == (H, W, 3))
+    _call("b200svd_vfi_merge", _ptr(warped0), _ptr(warped1), _ptr(fm), _ptr(res), res.stride(0), H, W, _ptr(pred),
+          _ptr(frame), _stream(), nbytes=H * W * (4.0 * 2 * (3 + 3 + 1 + 3) + 12 + 3), desc=f"{H}x{W}")
+    return pred, frame
+
+
+def vfi_pair_input(img0, img1, imgs, x8):
+    """img0, img1: fp32 [1, 3, H, W] contiguous -> imgs fp32 [4, 3, H, W] = [img0, flip(img0), img1, flip(img1)] and
+    x8 bf16 [4, H, W, 8] (channels 3..7 zero)."""
+    _, _, H, W = img0.shape
+    for t in (img0, img1):
+        assert t.dtype == torch.float32 and t.is_contiguous() and t.shape == (1, 3, H, W)
+    assert imgs.shape == (4, 3, H, W) and imgs.is_contiguous() and x8.shape == (4, H, W, 8) and x8.is_contiguous()
+    _call("b200svd_vfi_pair_input", _ptr(img0), _ptr(img1), H, W, _ptr(imgs), _ptr(x8), _stream(),
+          nbytes=H * W * (24.0 + 48 + 64), desc=f"{H}x{W}")
+    return imgs, x8
+
+
+def vfi_frames_to_bgr(frames, out=None):
+    """uint8 RGB [F, H, W, 3] contiguous -> fp32 BGR [F, 3, H, W] in [0, 1] (u / 255.0 rounded to float)."""
+    assert frames.dtype == torch.uint8 and frames.dim() == 4 and frames.shape[3] == 3 and frames.is_contiguous()
+    Fn, H, W, _ = frames.shape
+    if out is None:
+        out = torch.empty((Fn, 3, H, W), dtype=torch.float32, device=frames.device)
+    assert out.is_contiguous() and out.shape == (Fn, 3, H, W) and out.dtype == torch.float32
+    _call("b200svd_vfi_frames_to_bgr", _ptr(frames), Fn, H, W, _ptr(out), _stream(), nbytes=15.0 * frames.numel() / 3,
+          desc=f"{Fn}x{H}x{W}")
     return out
