@@ -292,11 +292,11 @@ int b200svd_frames_quantize(const float* x, float* out, int64_t n, void* stream)
  *   qkv: bf16 rows [2*pairs*h*w + 1][ldq], image-major, columns [q | k | v] each heads*32 wide; the last row is the
  *   padding token (the projections of LayerNorm(0)).  cor_embed: bf16 [h*w + 1][ldc], heads*8 columns, the last row
  *   the padding token.  Writes, for every real token, out = attn @ v (heads*32 columns) and motion =
- *   attn @ cor_embed - cor_embed (heads*8 columns).  Errors: qkv / cor_embed not 16-byte aligned or leading dims not
- *   multiples of 8.
+ *   attn @ cor_embed - cor_embed (heads*8 columns).  Errors: heads > 65535, 2*pairs > 65535, shift not 0 or 3,
+ *   qkv / cor_embed not 16-byte aligned, ldq / ldc not multiples of 8, or a leading dim narrower than its heads.
  * vfi_warp: warplayer.warp, grid_sample(bilinear, padding border, align_corners=True) at linspace grid + flow /
  *   ((size-1)/2).  Elements (n, c, y, x) of in / flow / out at the given element strides; flow points at its x channel
- *   (y channel one channel stride further).  in fp32 or bf16, out fp32 or bf16 (bf16 in needs bf16 out); h, w >= 2.
+ *   (y channel one channel stride further).  in and out both fp32 or both bf16; h, w >= 2 unless n*h*w == 0.
  * vfi_resize: F.interpolate(bilinear, align_corners=False, scale_factor = 2^factor_log2, factor_log2 in
  *   {-2, -1, 1, 2}) of fp32 in [n][c][h][w] (element strides), times mul, written (fp32 or bf16) or, with accumulate
  *   (fp32 only), added to out.

@@ -386,10 +386,12 @@ extern "C" {
 int b200svd_vfi_window_attn(const void* qkv, int64_t ldq, const void* cor_embed, int64_t ldc, void* out, int64_t ldo,
                             void* motion, int64_t ldm, int pairs, int h, int w, int heads, int shift, float scale,
                             void* stream) {
-  if (pairs < 1 || h < 1 || w < 1 || heads < 1 || heads > 65535 || 2 * pairs > 65535 || (shift != 0 && shift != 3)) {
-    set_error("b200svd_vfi_window_attn: pairs=%d h=%d w=%d heads=%d shift=%d out of range", pairs, h, w, heads, shift);
+  if (pairs < 0 || h < 0 || w < 0 || heads < 0 || heads > 65535 || pairs > 32767 || (shift != 0 && shift != 3)) {
+    set_error("b200svd_vfi_window_attn: pairs=%d h=%d w=%d heads=%d shift=%d out of range (heads <= 65535, "
+              "2*pairs <= 65535, shift 0 or 3)", pairs, h, w, heads, shift);
     return 1;
   }
+  if ((int64_t)pairs * h * w * heads == 0) return 0;
   if (!aligned(qkv, 16) || !aligned(cor_embed, 16) || ldq % 8 || ldc % 8 || ldq < 3 * heads * VHD ||
       ldc < heads * VMD || ldo < heads * VHD || ldm < heads * VMD) {
     set_error("b200svd_vfi_window_attn: qkv / cor_embed need 16-byte aligned bases and leading dims that are multiples "
@@ -416,27 +418,29 @@ int b200svd_vfi_window_attn(const void* qkv, int64_t ldq, const void* cor_embed,
 int b200svd_vfi_warp(const void* in, int in_bf16, int64_t isn, int64_t isc, int64_t isy, int64_t isx,
                      const float* flow, int64_t fsn, int64_t fsc, int64_t fsy, int64_t fsx, void* out, int out_bf16,
                      int64_t osn, int64_t osc, int64_t osy, int64_t osx, int n, int c, int h, int w, void* stream) {
-  if (n < 0 || c < 0 || h < 2 || w < 2) {
-    set_error("b200svd_vfi_warp: n=%d c=%d h=%d w=%d out of range (h, w >= 2)", n, c, h, w);
+  if (in_bf16 != out_bf16) {
+    set_error("b200svd_vfi_warp: in and out must both be fp32 or both bf16 (in_bf16=%d out_bf16=%d)", in_bf16,
+              out_bf16);
+    return 1;
+  }
+  if (n < 0 || c < 0 || h < 0 || w < 0) {
+    set_error("b200svd_vfi_warp: n=%d c=%d h=%d w=%d out of range", n, c, h, w);
     return 1;
   }
   const int64_t total = (int64_t)n * h * w;
   if (total == 0 || c == 0) return 0;
-  const VfiStr4 is{isn, isc, isy, isx}, fs{fsn, fsc, fsy, fsx}, os{osn, osc, osy, osx};
-  cudaStream_t st = (cudaStream_t)stream;
-  if (in_bf16 && out_bf16)
-    vfi_warp_kernel<<<vfi_blocks(total), VFI_THREADS, 0, st>>>((const __nv_bfloat16*)in, is, flow, fs,
-                                                           (__nv_bfloat16*)out, os, n, c, h, w);
-  else if (!in_bf16 && !out_bf16)
-    vfi_warp_kernel<<<vfi_blocks(total), VFI_THREADS, 0, st>>>((const float*)in, is, flow, fs, (float*)out, os, n, c, h,
-                                                           w);
-  else if (!in_bf16 && out_bf16)
-    vfi_warp_kernel<<<vfi_blocks(total), VFI_THREADS, 0, st>>>((const float*)in, is, flow, fs, (__nv_bfloat16*)out, os, n,
-                                                           c, h, w);
-  else {
-    set_error("b200svd_vfi_warp: a bf16 input needs a bf16 output");
+  if (h < 2 || w < 2) {  // the grid's (size - 1) / 2 normalisation
+    set_error("b200svd_vfi_warp: h=%d w=%d, both must be >= 2", h, w);
     return 1;
   }
+  const VfiStr4 is{isn, isc, isy, isx}, fs{fsn, fsc, fsy, fsx}, os{osn, osc, osy, osx};
+  cudaStream_t st = (cudaStream_t)stream;
+  if (in_bf16)
+    vfi_warp_kernel<<<vfi_blocks(total), VFI_THREADS, 0, st>>>((const __nv_bfloat16*)in, is, flow, fs,
+                                                           (__nv_bfloat16*)out, os, n, c, h, w);
+  else
+    vfi_warp_kernel<<<vfi_blocks(total), VFI_THREADS, 0, st>>>((const float*)in, is, flow, fs, (float*)out, os, n, c, h,
+                                                           w);
   B200_CHECK_LAUNCH("b200svd_vfi_warp");
   return 0;
 }
@@ -444,7 +448,7 @@ int b200svd_vfi_warp(const void* in, int in_bf16, int64_t isn, int64_t isc, int6
 int b200svd_vfi_resize(const float* in, int64_t isn, int64_t isc, int64_t isy, int64_t isx, void* out, int out_bf16,
                        int64_t osn, int64_t osc, int64_t osy, int64_t osx, int n, int c, int h, int w, int factor_log2,
                        float mul, int accumulate, void* stream) {
-  if (factor_log2 < -2 || factor_log2 > 2 || factor_log2 == 0 || n < 0 || c < 0 || h < 1 || w < 1 ||
+  if (factor_log2 < -2 || factor_log2 > 2 || factor_log2 == 0 || n < 0 || c < 0 || h < 0 || w < 0 ||
       (out_bf16 && accumulate)) {
     set_error("b200svd_vfi_resize: factor 2^%d (must be 1/4, 1/2, 2 or 4), n=%d c=%d h=%d w=%d, accumulate=%d "
               "(fp32 outputs only)", factor_log2, n, c, h, w, accumulate);

@@ -782,8 +782,8 @@ def _nchw_strides(t):
 
 def vfi_warp(inp, flow, out):
     """Backward warp (warplayer.warp): out = grid_sample(inp, linspace grid + flow, bilinear, border,
-    align_corners=True).  inp / out: [n, c, h, w] views with any element strides (fp32 or bf16; a bf16 input needs a
-    bf16 output), flow: [n, 2, h, w] fp32 view (x then y)."""
+    align_corners=True).  inp / out: [n, c, h, w] views with any element strides (both fp32 or both bf16), flow:
+    [n, 2, h, w] fp32 view (x then y)."""
     n, c, h, w = inp.shape
     assert out.shape == inp.shape and flow.shape == (n, 2, h, w) and flow.dtype == torch.float32
     ib, ob = inp.dtype == torch.bfloat16, out.dtype == torch.bfloat16

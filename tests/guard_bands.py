@@ -13,9 +13,10 @@ NAN = float("nan")
 
 class Guarded:
     """`view` ([rows, cols]) sits at row `pre` of a NaN-filled [pre + rows + post, ld] buffer, ld = cols rounded up
-    to 8 plus `pad` columns.  `flat=True`: a contiguous tensor of any shape inside a flat NaN buffer instead."""
+    to 8 plus `pad` columns, or the given `ld` with the view at column `col`.  `flat=True`: a contiguous tensor of any
+    shape inside a flat NaN buffer instead."""
 
-    def __init__(self, shape, dtype, dev, *, pre=3, post=5, pad=8, flat=False):
+    def __init__(self, shape, dtype, dev, *, pre=3, post=5, pad=8, flat=False, ld=None, col=0):
         assert pad % 8 == 0
         self.dtype = dtype
         if flat:
@@ -24,10 +25,12 @@ class Guarded:
             self.view = self.buf[8 * pre:8 * pre + n].view(shape)
         else:
             rows, cols = shape
-            ld = -(-cols // 8) * 8 + pad
+            if ld is None:
+                ld = -(-cols // 8) * 8 + pad
+            assert col + cols <= ld
             self.buf = torch.full((pre + rows + post, ld), NAN, dtype=dtype, device=dev)
-            self.view = self.buf[pre:pre + rows, :cols]
-        assert self.view.data_ptr() % 16 == 0
+            self.view = self.buf[pre:pre + rows, col:col + cols]
+        assert self.view.data_ptr() % 16 == 0 or col, "views at column 0 start 16-byte aligned"
 
     def fill(self, values):
         self.view.copy_(values)

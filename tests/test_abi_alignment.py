@@ -240,3 +240,112 @@ def test_group_norm_empty_and_zero_width_in_subprocess(lib):
     r = subprocess.run([sys.executable, "-c", _GN_EMPTY_SCRIPT, root], capture_output=True, text=True, timeout=300)
     assert r.returncode == 0 and r.stdout.strip() == "ok", \
         f"exit {r.returncode}\nstdout: {r.stdout[-2000:]}\nstderr: {r.stderr[-2000:]}"
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# interpolation-stage entry points (csrc/vfi.cu)
+# ---------------------------------------------------------------------------------------------------------------------
+def _win(lib, qkv=X, ldq=1536, ce=Y, ldc=128, ldo=512, ldm=128, pairs=2, h=45, w=80, heads=16, shift=0):
+    return lib.b200svd_vfi_window_attn(qkv, ldq, ce, ldc, Z, ldo, Z + 0x100000, ldm, pairs, h, w, heads, shift,
+                                       0.17677669, None)
+
+
+def _warp(lib, in_bf16=1, out_bf16=1, n=2, c=32, h=45, w=80):
+    return lib.b200svd_vfi_warp(X, in_bf16, h * w * c, 1, w * c, c, Y, 2 * h * w, h * w, w, 1, Z, out_bf16,
+                                h * w * c, 1, w * c, c, n, c, h, w, None)
+
+
+def _resize(lib, log2=-1, out_bf16=0, accumulate=0, n=2, c=4, h=90, w=160):
+    return lib.b200svd_vfi_resize(X, c * h * w, h * w, w, 1, Y, out_bf16, c * h * w, h * w, w, 1, n, c, h, w, log2,
+                                  1.0, accumulate, None)
+
+
+def _dwconv(lib, x=X, y=Y, n=4, h=45, w=80, c=2048):
+    return lib.b200svd_vfi_dwconv_gelu(x, y, n, h, w, c, GAMMA, BETA, None)
+
+
+def _gather(lib, pairs=2, h=45, w=80, c=512, ldm=512, lda=512, ldo=136):
+    return lib.b200svd_vfi_head_gather(X, ldm, Y, lda, pairs, h, w, c, Z, ldo, None)
+
+
+def _merge(lib, h=720, w=1280, ldr=3):
+    return lib.b200svd_vfi_merge(X, Y, Z, GAMMA, ldr, h, w, BETA, BETA + 0x1000000, None)
+
+
+def _pair(lib, h=720, w=1280, x8=Z):
+    return lib.b200svd_vfi_pair_input(X, Y, h, w, GAMMA, x8, None)
+
+
+VFI_EMPTY = {
+    "window_attn_pairs0": lambda lib: _win(lib, pairs=0),
+    "window_attn_h0": lambda lib: _win(lib, h=0),
+    "window_attn_w0": lambda lib: _win(lib, w=0),
+    "window_attn_heads0": lambda lib: _win(lib, heads=0),
+    "warp_n0": lambda lib: _warp(lib, n=0),
+    "warp_c0": lambda lib: _warp(lib, c=0),
+    "warp_h0": lambda lib: _warp(lib, h=0),
+    "warp_w0_fp32": lambda lib: _warp(lib, in_bf16=0, out_bf16=0, w=0),
+    "resize_n0": lambda lib: _resize(lib, n=0),
+    "resize_h0": lambda lib: _resize(lib, h=0),
+    "resize_w0_up": lambda lib: _resize(lib, log2=2, w=0),
+    "resize_h3_quarter": lambda lib: _resize(lib, log2=-2, h=3),          # floor(3 / 4) = 0 output rows
+    "dwconv_n0": lambda lib: _dwconv(lib, n=0),
+    "dwconv_c0": lambda lib: _dwconv(lib, c=0),
+    "head_gather_pairs0": lambda lib: _gather(lib, pairs=0),
+    "head_gather_h0": lambda lib: _gather(lib, h=0),
+    "merge_h0": lambda lib: _merge(lib, h=0),
+    "merge_w0": lambda lib: _merge(lib, w=0),
+    "pair_input_h0": lambda lib: _pair(lib, h=0),
+    "frames_to_bgr_n0": lambda lib: lib.b200svd_vfi_frames_to_bgr(X, 0, 720, 1280, Y, None),
+    "frames_to_bgr_w0": lambda lib: lib.b200svd_vfi_frames_to_bgr(X, 3, 720, 0, Y, None),
+}
+
+
+@pytest.mark.parametrize("case", list(VFI_EMPTY))
+def test_vfi_empty_output_returns_zero(lib, case):
+    rc = VFI_EMPTY[case](lib)
+    assert rc == 0, lib.b200svd_last_error().decode()
+
+
+VFI_REJECT = {
+    # (call, words the message must contain)
+    "window_attn_heads_65536": (lambda lib: _win(lib, heads=65536, ldq=3 * 65536 * 32, ldc=65536 * 8,
+                                                 ldo=65536 * 32, ldm=65536 * 8), ("heads=65536",)),
+    "window_attn_pairs_32768": (lambda lib: _win(lib, pairs=32768), ("pairs=32768",)),
+    "window_attn_negative_h": (lambda lib: _win(lib, h=-1), ("h=-1",)),
+    "window_attn_shift_1": (lambda lib: _win(lib, shift=1), ("shift=1",)),
+    "window_attn_shift_7": (lambda lib: _win(lib, shift=7), ("shift=7",)),
+    "window_attn_qkv_misaligned": (lambda lib: _win(lib, qkv=X + 8), ("align",)),
+    "window_attn_ce_misaligned": (lambda lib: _win(lib, ce=Y + 2), ("align",)),
+    "window_attn_ldq_odd": (lambda lib: _win(lib, ldq=1540), ("multiples of 8",)),
+    "window_attn_ldq_narrow": (lambda lib: _win(lib, ldq=1528), ("heads",)),
+    "window_attn_ldc_narrow": (lambda lib: _win(lib, ldc=120), ("heads",)),
+    "window_attn_ldo_narrow": (lambda lib: _win(lib, ldo=511), ("heads",)),
+    "window_attn_ldm_narrow": (lambda lib: _win(lib, ldm=127), ("heads",)),
+    "warp_bf16_in_fp32_out": (lambda lib: _warp(lib, in_bf16=1, out_bf16=0), ("fp32 or both bf16",)),
+    "warp_fp32_in_bf16_out": (lambda lib: _warp(lib, in_bf16=0, out_bf16=1), ("fp32 or both bf16",)),
+    "warp_w1": (lambda lib: _warp(lib, w=1), ("w=1",)),
+    "warp_h1": (lambda lib: _warp(lib, h=1), ("h=1",)),
+    "warp_negative_c": (lambda lib: _warp(lib, c=-1), ("c=-1",)),
+    "resize_factor_0": (lambda lib: _resize(lib, log2=0), ("factor",)),
+    "resize_factor_8": (lambda lib: _resize(lib, log2=3), ("factor",)),
+    "resize_factor_1_8": (lambda lib: _resize(lib, log2=-3), ("factor",)),
+    "resize_bf16_accumulate": (lambda lib: _resize(lib, out_bf16=1, accumulate=1), ("accumulate=1",)),
+    "resize_negative_h": (lambda lib: _resize(lib, h=-4), ("h=-4",)),
+    "dwconv_c_12": (lambda lib: _dwconv(lib, c=12), ("c=12", "multiple of 8")),
+    "dwconv_x_misaligned": (lambda lib: _dwconv(lib, x=X + 8), ("align",)),
+    "dwconv_y_misaligned": (lambda lib: _dwconv(lib, y=Y + 2), ("align",)),
+    "head_gather_c_6": (lambda lib: _gather(lib, c=6, ldm=8, lda=8), ("c=6",)),
+    "head_gather_ldo_narrow": (lambda lib: _gather(lib, ldo=127), ("leading dims",)),
+    "head_gather_ldm_narrow": (lambda lib: _gather(lib, ldm=504), ("leading dims",)),
+    "head_gather_lda_narrow": (lambda lib: _gather(lib, lda=504), ("leading dims",)),
+    "merge_ldr_2": (lambda lib: _merge(lib, ldr=2), ("ldr=2",)),
+    "pair_input_x8_misaligned": (lambda lib: _pair(lib, x8=Z + 8), ("align",)),
+    "frames_to_bgr_negative_n": (lambda lib: lib.b200svd_vfi_frames_to_bgr(X, -1, 720, 1280, Y, None), ("n=-1",)),
+}
+
+
+@pytest.mark.parametrize("case", list(VFI_REJECT))
+def test_vfi_rejects_out_of_range_arguments(lib, case):
+    call, words = VFI_REJECT[case]
+    _assert_error(lib, call(lib), *words)

@@ -16,87 +16,14 @@ import torch.nn.functional as F
 
 pytestmark = pytest.mark.gpu
 
+from vfi_refs import ref_warp as _ref_warp, ref_window_attn as _ref_window_attn, warp_bound
+
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
 
 # ---------------------------------------------------------------------------------------------------------------
 # window attention
 # ---------------------------------------------------------------------------------------------------------------
-def _ref_window_attn(q, k, v, ce, pairs, h, w, heads, shift):
-    """MotionFormerBlock / InterFrameAttention arithmetic (feature_extractor.py:7-61, 146-172, 213-277) in float64 on
-    token tensors [2*pairs, h, w, C] (q, k, v) and [h, w, Cm] (ce); padding tokens take the given pad rows."""
-    q, k, v, ce = (t.double() for t in (q, k, v, ce))
-    (qp, kp, vp, cep) = (t[-1] for t in (q, k, v, ce))
-    n = 2 * pairs
-    qi, ki, vi = (t[:-1].view(n, h, w, -1) for t in (q, k, v))
-    cei = ce[:-1].view(1, h, w, -1).expand(n, h, w, -1)
-    ws = 7
-    ph, pw = -(-h // ws) * ws - h, -(-w // ws) * ws - w
-    H, W = h + ph, w + pw
-
-    def pad(t, fill):
-        out = fill.view(1, 1, 1, -1).expand(t.shape[0], H, W, -1).clone()
-        out[:, ph // 2:ph // 2 + h, pw // 2:pw // 2 + w] = t
-        return out
-
-    qx, kx, vx, cx = pad(qi, qp), pad(ki, kp), pad(vi, vp), pad(cei, cep)
-
-    def part(t):
-        b, _, _, c = t.shape
-        return t.view(b, H // ws, ws, W // ws, ws, c).permute(0, 1, 3, 2, 4, 5).reshape(-1, ws * ws, c)
-
-    mask = None
-    if ph or pw:
-        img = torch.zeros((1, H, W, 1))
-        cnt = 0
-        for hs in (slice(0, ph // 2), slice(ph // 2, h + ph // 2), slice(h + ph // 2, None)):
-            for wsl in (slice(0, pw // 2), slice(pw // 2, w + pw // 2), slice(w + pw // 2, None)):
-                img[:, hs, wsl, :] = cnt
-                cnt += 1
-        mw = part(img).squeeze(-1)
-        mask = mw.unsqueeze(1) - mw.unsqueeze(2)
-        mask = mask.masked_fill(mask != 0, -100.0).masked_fill(mask == 0, 0.0)
-    if shift:
-        qx, kx, vx, cx = (torch.roll(t, (-shift, -shift), (1, 2)) for t in (qx, kx, vx, cx))
-        sm = torch.zeros((1, H, W, 1))
-        cnt = 0
-        for hs in (slice(0, -ws), slice(-ws, -shift), slice(-shift, None)):
-            for wsl in (slice(0, -ws), slice(-ws, -shift), slice(-shift, None)):
-                sm[:, hs, wsl, :] = cnt
-                cnt += 1
-        mw = part(sm).squeeze(-1)
-        sm = mw.unsqueeze(1) - mw.unsqueeze(2)
-        sm = sm.masked_fill(sm != 0, -100.0).masked_fill(sm == 0, 0.0)
-        if mask is not None:
-            sm = sm.masked_fill(mask != 0, -100.0)
-        mask = sm
-    Q, K, V, CE = part(qx), part(kx), part(vx), part(cx)
-    nwB = Q.shape[0]
-    K = torch.cat([K[nwB // 2:], K[:nwB // 2]])
-    V = torch.cat([V[nwB // 2:], V[:nwB // 2]])
-    N = ws * ws
-    Qh = Q.view(nwB, N, heads, -1).permute(0, 2, 1, 3)
-    Kh = K.view(nwB, N, heads, -1).permute(0, 2, 1, 3)
-    Vh = V.view(nwB, N, heads, -1).permute(0, 2, 1, 3)
-    Ch = CE.view(nwB, N, heads, -1).permute(0, 2, 1, 3)
-    attn = (Qh @ Kh.transpose(-2, -1)) * 32 ** -0.5
-    if mask is not None:
-        nW = mask.shape[0]
-        attn = (attn.view(nwB // nW, nW, heads, N, N) + mask.double().unsqueeze(1).unsqueeze(0)).view(-1, heads, N, N)
-    attn = attn.softmax(-1)
-    x = (attn @ Vh).transpose(1, 2).reshape(nwB, N, -1)
-    m = (attn @ Ch).transpose(1, 2).reshape(nwB, N, -1) - CE
-
-    def rev(t):
-        c = t.shape[-1]
-        t = t.view(n, H // ws, W // ws, ws, ws, c).permute(0, 1, 3, 2, 4, 5).reshape(n, H, W, c)
-        if shift:
-            t = torch.roll(t, (shift, shift), (1, 2))
-        return t[:, ph // 2:ph // 2 + h, pw // 2:pw // 2 + w].reshape(n * h * w, c)
-
-    return rev(x), rev(m)
-
-
 @pytest.mark.parametrize("h,w,heads,shift", [(14, 28, 8, 0), (14, 28, 8, 3), (12, 20, 8, 0), (12, 20, 8, 3),
                                              (6, 10, 16, 0), (6, 10, 16, 3), (7, 14, 16, 3), (9, 5, 8, 3)])
 def test_window_attn(cuda_dev, h, w, heads, shift):
@@ -123,14 +50,6 @@ def test_window_attn(cuda_dev, h, w, heads, shift):
 # ---------------------------------------------------------------------------------------------------------------
 # warp, resize
 # ---------------------------------------------------------------------------------------------------------------
-def _ref_warp(x, flow):
-    n, c, h, w = x.shape
-    gx = torch.linspace(-1.0, 1.0, w, dtype=torch.float64).view(1, 1, w).expand(n, h, w)
-    gy = torch.linspace(-1.0, 1.0, h, dtype=torch.float64).view(1, h, 1).expand(n, h, w)
-    g = torch.stack([gx + flow[:, 0].double() / ((w - 1.0) / 2.0), gy + flow[:, 1].double() / ((h - 1.0) / 2.0)], -1)
-    return F.grid_sample(x.double(), g, mode="bilinear", padding_mode="border", align_corners=True)
-
-
 @pytest.mark.parametrize("n,c,h,w,bf16", [(2, 3, 96, 160, False), (2, 32, 48, 80, True), (2, 512, 6, 10, True),
                                           (2, 3, 720, 1280, False)])
 def test_warp(cuda_dev, n, c, h, w, bf16):
@@ -155,8 +74,7 @@ def test_warp(cuda_dev, n, c, h, w, bf16):
     torch.cuda.synchronize()
     ref = _ref_warp(x.double(), flow)
     got = out.double().cpu()
-    # a coordinate error of one fp32 ulp of the (unnormalised) position moves the sample by |gradient| * ulp
-    tol = (2.0 ** -8 * ref.abs() if bf16 else 0) + 2e-5 * max(h, w)
+    tol = warp_bound(ref, flow, bf16)                          # derived in tests/vfi_refs.py
     err = (got - ref).abs()
     assert (err <= tol).all(), f"max err {err.max():.3g}"
     if bf16:
