@@ -400,9 +400,13 @@ def test_layer_norm_branches(cuda_dev, case):
     """ldx > C, ldy > C (NaN pad columns); rows ragged against 8 warps x rows per warp; fvec with rows_per_frame,
     with and without xsum; gamma / beta / fvec at a 4-byte offset (scalar fallback, same bound); the CLIP ln_post
     layout (3 class rows at a row stride of 257 x 1280); constant rows give exactly bf16(beta)."""
-    from streamingt2v_b200 import ops
-    dev = cuda_dev
     rows, C, o = LN_CASES[case]
+    _ln_case(cuda_dev, case, rows, C, o)
+
+
+def _ln_case(dev, case, rows, C, o, eps=1e-5):
+    """One LayerNorm launch of `rows` x C with the options of LN_CASES, run twice, against float64 in row chunks."""
+    from streamingt2v_b200 import ops
     seed = rows * 7 + C
     step = o.get("stride_rows", 1)
     vals = _randn((rows, C), seed, dev, 1.5, 0.3)
@@ -437,44 +441,52 @@ def test_layer_norm_branches(cuda_dev, case):
         XS = _out((rows, C), torch.bfloat16, dev, pad=16)
         kw["xsum"] = XS.view
     Y = _out((rows, C), torch.bfloat16, dev, pad=8)
-    ops.layer_norm(x, gamma, beta, 1e-5, out=Y.view, **kw)
+    ops.layer_norm(x, gamma, beta, eps, out=Y.view, **kw)
     torch.cuda.synchronize()
     Y.check(case)
     first = Y.view.clone()
     if XS is not None:
         XS.check(case + " xsum")
         first_xs = XS.view.clone()
-    ops.layer_norm(x, gamma, beta, 1e-5, out=Y.view, **kw)
+    ops.layer_norm(x, gamma, beta, eps, out=Y.view, **kw)
     torch.cuda.synchronize()
     _assert_same_bits(first, Y.view, case)
     if XS is not None:
         _assert_same_bits(first_xs, XS.view, case + " xsum")
+    del first
+    if XS is not None:
+        del first_xs
 
-    if fv is not None:
-        f_rows = fv.repeat_interleave(kw["rows_per_frame"], 0)[:rows]
-        if XS is not None:
-            xs_ref = (x.float() + f_rows).bfloat16()
-            assert torch.equal(XS.view, xs_ref), f"{case}: xsum != bf16(x + fvec)"
-            v = xs_ref.double()
-        else:
-            v = x.double() + f_rows.double()
-    else:
-        v = x.double()
-    mean = v.mean(1, keepdim=True)
-    rstd = 1.0 / torch.sqrt((v - mean).pow(2).mean(1, keepdim=True) + _f32(1e-5))
     g, b = gamma.double(), beta.double()
-    xg = (v - mean) * rstd * g
-    pre = xg + b
-    dev_ = xg.abs() + rstd * g.abs() * v.abs().mean(1, keepdim=True)
-    if kw["silu"]:
-        ref = F.silu(pre)
-        bound = 2 ** -8 * ref.abs() + 1.1 * (2 ** -16 * dev_ + 2 ** -20 * b.abs()) + 2 ** -16 * pre.abs()
-    else:
-        ref = pre
-        bound = 2 ** -8 * ref.abs() + 2 ** -16 * dev_ + 2 ** -20 * b.abs()
+    acc = _Rows()
+    for r0, r1 in _row_chunks(rows, C):
+        xr = x[r0:r1]
+        if fv is not None:
+            f_rows = fv[torch.arange(r0, r1, device=dev) // kw["rows_per_frame"]]
+            if XS is not None:
+                xs_ref = (xr.float() + f_rows).bfloat16()
+                assert torch.equal(XS.view[r0:r1], xs_ref), f"{case}: xsum != bf16(x + fvec)"
+                v = xs_ref.double()
+            else:
+                v = xr.double() + f_rows.double()
+        else:
+            v = xr.double()
+        mean = v.mean(1, keepdim=True)
+        rstd = 1.0 / torch.sqrt((v - mean).pow(2).mean(1, keepdim=True) + _f32(eps))
+        xg = (v - mean) * rstd * g
+        pre = xg + b
+        dev_ = xg.abs() + rstd * g.abs() * v.abs().mean(1, keepdim=True)
+        if kw["silu"]:
+            ref = F.silu(pre)
+            bound = 2 ** -8 * ref.abs() + 1.1 * (2 ** -16 * dev_ + 2 ** -20 * b.abs()) + 2 ** -16 * pre.abs()
+        else:
+            ref = pre
+            bound = 2 ** -8 * ref.abs() + 2 ** -16 * dev_ + 2 ** -20 * b.abs()
+        acc.add(Y.view[r0:r1], ref, bound)
+    if not kw["silu"]:
         for r in const_rows:
             assert torch.equal(Y.view[r], beta.bfloat16()), f"{case}: constant row {r} is not bf16(beta)"
-    _check_bound(Y.view, ref, bound, f"{case} rows{rows}", "layernorm")
+    acc.finish(f"{case} rows{rows}", "layernorm")
 
 
 # ---------------------------------------------------------------------------------------------------------------------

@@ -6,8 +6,8 @@ Census.  CENSUS is the literal list of distinct launches (tests/vfi_census.py st
 test_census_matches_vfi_py recomputes it on the CPU (the network on the `meta` device with shape-only ops), so a
 launch shape added to vfi.py fails here until it is added to the table, and with it to the replays below.
 
-GEMM bound.  Operands are bf16, so every product x*w is exact in fp32; the kernel sums n = K * taps of them (plus the
-bias) in fp32.  Each addition rounds by at most 2^-24 relative, so the sum is within gamma_n S, gamma_n = n 2^-24 /
+GEMM bound (tests/gemm_replay.py, which the denoiser's replays share).  Operands are bf16, so every product x*w is
+exact in fp32; the kernel sums n = K * taps of them (plus the bias) in fp32.  Each addition rounds by at most 2^-24 relative, so the sum is within gamma_n S, gamma_n = n 2^-24 /
 (1 - n 2^-24) <= n 2^-23, of the exact one, S = sum |x| |w| + |bias| (a second float64 launch on |x|, |w|).  The
 epilogue adds a few roundings more (bias, PReLU multiply, residual add: 4 more terms of 2^-23 S, the residual's
 magnitude added to S), and a PReLU slope a scales the negative side by |a|.  The bf16 store rounds to nearest, 2^-8
@@ -26,6 +26,7 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from gemm_replay import bits, free, gemm_bound, launch, ref_gemm, replay
 from guard_bands import Guarded, _check_bound
 from vfi_census import GEMM_OPS, census
 from vfi_refs import ref_warp, ref_window_attn
@@ -155,48 +156,13 @@ def test_census_matches_vfi_py():
 GEMM = [c for c in CENSUS if c[0] in GEMM_OPS]
 
 
-def _free():
-    torch.cuda.synchronize()
-    torch.cuda.empty_cache()
-
-
-def _bits(t):
-    return t.view({2: torch.int16, 4: torch.int32}[t.element_size()])
-
-
 # ---------------------------------------------------------------------------------------------------------------------
 # every GEMM launch of the census
 # ---------------------------------------------------------------------------------------------------------------------
-def _ref_gemm(op, x, wt, extra):
-    """float64 op on x ([rows, K] or NHWC) with wt in torch layout -> rows [M, N]."""
-    if op == "linear":
-        return x @ wt.t()
-    xc = x.permute(0, 3, 1, 2)
-    if op == "conv3x3":
-        y = F.conv2d(xc, wt, padding=1)
-    elif op == "conv3x3_s2":
-        y = F.conv2d(xc, wt, stride=2, padding=1)
-    elif op == "conv3x3_strided":
-        s, d = extra
-        y = F.conv2d(xc, wt, stride=s, padding=d, dilation=d)
-    else:
-        y = F.conv_transpose2d(xc, wt, stride=2, padding=1)
-    return y.permute(0, 2, 3, 1).reshape(-1, y.shape[1])
-
-
-def _launch(op, x, w, b, out, extra, epi):
-    from streamingt2v_b200 import ops
-    if op == "conv3x3_strided":
-        ops.conv3x3_strided(x, w, b, stride=extra[0], dilation=extra[1], out=out, **epi)
-    else:
-        getattr(ops, op)(x, w, b, out=out, **epi)
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("idx", range(len(GEMM)), ids=[f"{i:02d}-{c[0]}-{'x'.join(map(str, c[1]))}-n{c[8][1]}"
                                                        f"-ld{c[9]}-col{c[10]}" for i, c in enumerate(GEMM)])
 def test_gemm_launch_fp64(cuda_dev, idx):
-    from streamingt2v_b200 import ops
     from streamingt2v_b200._lib import ACT_PRELU
     from streamingt2v_b200.vfi import pack_deconv
     op, xs, xld, ws, act, f32, prelu, res_ld, os_, old, col, extra = GEMM[idx]
@@ -229,24 +195,11 @@ def test_gemm_launch_fp64(cuda_dev, idx):
         # the skip half of the concat, written before the deconv by copy2d, must come through bitwise
         O.buf[16:16 + rows, n:2 * n] = torch.randn((rows, n), generator=g, device=dev).to(O.dtype)
     O.snapshot()
-    schedules = [None] if prelu else [0, 1, None]
-    outs = []
-    for sched in schedules:
-        prev = ops.gemm_schedule(sched) if sched is not None else None
-        try:
-            for _ in range(2):
-                _launch(op, X.view, w, b, O.view, extra, epi)
-                torch.cuda.synchronize()
-                O.check(f"{op} {xs} schedule {sched}")
-                outs.append(O.view.clone())
-        finally:
-            if prev is not None:
-                ops.gemm_schedule(prev)
-    for o in outs[1:]:
-        assert torch.equal(_bits(o), _bits(outs[0])), "reruns / schedules differ bitwise"
+    out = replay(lambda: launch(op, X.view, w, b, O.view, extra, epi), O, f"{op} {xs}",
+                 schedules=(None,) if prelu else (0, 1, None))
     x64 = X.view.double()
-    v = _ref_gemm(op, x64, wt, extra) + b.double()
-    s_abs = _ref_gemm(op, x64.abs(), wt.abs(), extra) + b.double().abs()
+    v = ref_gemm(op, x64, wt, extra) + b.double()
+    s_abs = ref_gemm(op, x64.abs(), wt.abs(), extra) + b.double().abs()
     del x64
     amp = 1.0
     if prelu:
@@ -258,10 +211,10 @@ def test_gemm_launch_fp64(cuda_dev, idx):
     if res_ld:
         ref = ref + res.double()
         s_abs = s_abs + res.double().abs()
-    bound = (2.0 ** -23 if f32 else 2.0 ** -8) * ref.abs() + (K * taps + 4) * 2.0 ** -23 * amp * s_abs
-    _check_bound(outs[0], ref, bound, f"{op} {xs}->{n} ld{old} col{col}", f"gemm {op}{' prelu' if prelu else ''}")
-    del v, s_abs, ref, bound, outs, X, O
-    _free()
+    bound = gemm_bound(ref, s_abs, K * taps, f32, amp)
+    _check_bound(out, ref, bound, f"{op} {xs}->{n} ld{old} col{col}", f"gemm {op}{' prelu' if prelu else ''}")
+    del v, s_abs, ref, bound, out, X, O
+    free()
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -299,7 +252,7 @@ def test_window_attn_production(cuda_dev, h, w, heads, shift, pad, sharp):
         O.check("attn@v")
         M.check("motion")
         outs.append((O.view.clone(), M.view.clone()))
-    assert all(torch.equal(_bits(a), _bits(b)) for a, b in zip(outs[0], outs[1])), "reruns differ bitwise"
+    assert all(torch.equal(bits(a), bits(b)) for a, b in zip(outs[0], outs[1])), "reruns differ bitwise"
     rx, rm = ref_window_attn(qkv[:, :C], qkv[:, C:2 * C], qkv[:, 2 * C:], ce, pairs, h, w, heads, shift)
     # fp32 logits: 32 products summed, |error| <= 32 2^-23 sum|q||k| scale + one rounding; a logit error e moves
     # softmax-weighted sums of v by at most 2 e max|v|
@@ -310,7 +263,7 @@ def test_window_attn_production(cuda_dev, h, w, heads, shift, pad, sharp):
         bound = 2.0 ** -8 * ref.abs() + 2e-4 * (1 + ref.abs()) + 2 * e * vmax
         _check_bound(got, ref, bound, f"{h}x{w} heads{heads} shift{shift} pad{pad} sharp{sharp} {name}",
                      "window_attn", l2=2 ** -7)
-    _free()
+    free()
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -336,7 +289,7 @@ def _check_strided(buf, snap, view, name):
     assert torch.isfinite(view).all(), f"{name}: unwritten or non-finite output elements"
     inside = torch.zeros(buf.shape, dtype=torch.bool, device=buf.device)
     inside.as_strided(view.shape, view.stride(), view.storage_offset()).fill_(True)
-    n_bad = (_bits(buf)[~inside] != _bits(snap)[~inside]).sum().item()
+    n_bad = (bits(buf)[~inside] != bits(snap)[~inside]).sum().item()
     assert n_bad == 0, f"{name}: {n_bad} elements outside the output view were written"
 
 
@@ -382,12 +335,12 @@ def test_warp_production(cuda_dev, idx):
         torch.cuda.synchronize()
         _check_strided(obuf, snap, out, "warp")
         outs.append(out.clone())
-    assert torch.equal(_bits(outs[0]), _bits(outs[1]))
+    assert torch.equal(bits(outs[0]), bits(outs[1]))
     ref = ref_warp(xin, flow)
     _check_bound(outs[0], ref, warp_bound(ref, flow, odt == "bfloat16"),
                  f"{n}x{c}x{h}x{w} {odt} in+{il[1]} flow+{fl[1]} out+{ol[1]}", "warp")
     del outs, ref, obuf, snap
-    _free()
+    free()
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -419,7 +372,7 @@ def _resize_case(dev, shape, il, odt, ol, log2, mul, acc, seed):
     bound = (2.0 ** -8 * ref.abs() if odt == "bfloat16" else 0) + 4e-6 * (ref.abs() + 10 * abs(mul))
     _check_bound(out, ref, bound, f"{shape} x2^{log2} mul{mul} acc{acc} {odt} in+{il[1]} out+{ol[1]}", "resize")
     del obuf, snap, ref
-    _free()
+    free()
 
 
 @pytest.mark.gpu
@@ -468,12 +421,12 @@ def test_dwconv_gelu_production(cuda_dev, h, w, c):
         torch.cuda.synchronize()
         O.check("dwconv_gelu")
         outs.append(O.view.clone())
-    assert torch.equal(_bits(outs[0]), _bits(outs[1]))
+    assert torch.equal(bits(outs[0]), bits(outs[1]))
     ref = F.gelu(F.conv2d(X.view.double().permute(0, 3, 1, 2), wt.double(), b.double(), padding=1, groups=c))
     ref = ref.permute(0, 2, 3, 1).reshape(-1, c)
     # 9 fp32 fmas and the bias (a few 2^-24 of sum |x w| <= 3 max|x|), erff within 2 ulp; then one bf16 rounding
     _check_bound(outs[0], ref, 2.0 ** -8 * ref.abs() + 1e-5, f"{h}x{w}x{c}", "dwconv")
-    _free()
+    free()
 
 
 @pytest.mark.gpu
@@ -499,7 +452,7 @@ def test_head_gather_production(cuda_dev, h, w, c, ld):
     cat = torch.cat([0.5 * m4[:pairs], 0.5 * m4[pairs:], a4[:pairs], a4[pairs:]], 1)
     ref = F.pixel_shuffle(F.pixel_shuffle(cat, 2), 2).permute(0, 2, 3, 1).reshape(-1, c // 4)
     assert torch.equal(O.view.double(), ref)
-    _free()
+    free()
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -533,7 +486,7 @@ def test_merge_720x1280(cuda_dev):
     _check_bound(P.view[0], ref, torch.full_like(ref, 1e-6), "720x1280", "merge")
     ref8 = (P.view[0].cpu().numpy().transpose(1, 2, 0) * 255.0).astype(np.uint8)[:, :, ::-1]
     assert np.array_equal(frame.cpu().numpy(), ref8)
-    _free()
+    free()
 
 
 @pytest.mark.gpu
