@@ -80,9 +80,11 @@ class Recorder:
             n, h, wd, _ = x.shape
             return r._gemm("conv3x3", x, w, bias, n * h * wd, w.shape[1], out, **epi)
 
-        def conv3x3_s2(x, w, bias=None, *, out=None, **epi):
+        def conv3x3_s2(x, w, bias=None, *, out=None, pad_after_only=False, **epi):
+            # the autoencoder's padding (tests/vae_clip_census.py) is its own op name: the record layout stays
+            op = "conv3x3_s2_pad_after" if pad_after_only else "conv3x3_s2"
             n, h, wd, _ = x.shape
-            return r._gemm("conv3x3_s2", x, w, bias, n * (h // 2) * (wd // 2), w.shape[1], out, **epi)
+            return r._gemm(op, x, w, bias, n * (h // 2) * (wd // 2), w.shape[1], out, **epi)
 
         def tconv3(x, w, bias=None, *, out=None, **epi):
             b, t, p, _ = x.shape

@@ -1,6 +1,6 @@
 """TEST INFRASTRUCTURE — replaying a census GEMM launch against float64: the reference op, the launch, the bound, the
-rerun / schedule / epilogue-body comparison.  Shared by tests/test_vfi_launches_gpu.py and
-tests/test_denoiser_launches_gpu.py.
+rerun / schedule / epilogue-body comparison.  Shared by tests/test_vfi_launches_gpu.py,
+tests/test_denoiser_launches_gpu.py and tests/test_vae_clip_launches_gpu.py.
 
 Bound.  Operands are bf16, so every product x*w is exact in fp32; the kernel sums n = K * taps of them (plus the
 bias) in fp32.  Each addition rounds by at most 2^-24 relative, so the sum is within gamma_n S, gamma_n = n 2^-24 /
@@ -35,6 +35,9 @@ def ref_gemm(op, x, wt, extra=()):
         y = F.conv2d(xc, wt, padding=1)
     elif op == "conv3x3_s2":
         y = F.conv2d(xc, wt, stride=2, padding=1)
+    elif op == "conv3x3_s2_pad_after":
+        # the autoencoder's Downsample: zero pad after (bottom and right) only, then a padding-0 stride-2 conv
+        y = F.conv2d(F.pad(xc, (0, 1, 0, 1)), wt, stride=2)
     elif op == "conv3x3_strided":
         s, d = extra
         y = F.conv2d(xc, wt, stride=s, padding=d, dilation=d)
@@ -47,6 +50,8 @@ def launch(op, x, w, b, out, extra, epi):
     from streamingt2v_b200 import ops
     if op == "conv3x3_strided":
         ops.conv3x3_strided(x, w, b, stride=extra[0], dilation=extra[1], out=out, **epi)
+    elif op == "conv3x3_s2_pad_after":
+        ops.conv3x3_s2(x, w, b, out=out, pad_after_only=True, **epi)
     else:
         getattr(ops, op)(x, w, b, out=out, **epi)
 
