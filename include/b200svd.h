@@ -332,6 +332,18 @@ int b200svd_vfi_merge(const float* warped0, const float* warped1, const float* f
 int b200svd_vfi_pair_input(const float* img0, const float* img1, int h, int w, float* imgs, void* x8, void* stream);
 int b200svd_vfi_frames_to_bgr(const void* frames, int64_t n, int h, int w, float* out, void* stream);
 
+/* ---- PIL's BICUBIC resize of uint8 RGB frames (the enhance stage's inputs, inference_i2v.py:194-199) -----------------
+ * uint8 [n][h_in][w_in][3] -> uint8 [n][h_out][w_out][3], equal byte for byte to Pillow's `Image.resize((w_out, h_out))`
+ * with BICUBIC: a horizontal pass (skipped when w_out == w_in) into `workspace` (uint8 [n][h_in][w_out][3], needed only
+ * when both axes change), then a vertical pass (skipped when h_out == h_in); both unchanged is a device copy.  Per
+ * axis, DEVICE arrays computed on the host once per (in, out) size pair (ops.bicubic_taps): bounds int32
+ * [out][2] = (first source index, tap count), 8-byte aligned, and taps int32 [out][k] = the coefficients in 2^-22
+ * units, zero past each tap count.  Each output sample is clip((2^21 + sum taps * source) >> 22, 0, 255) in int32.
+ * out must not overlap x or workspace.  Returns 0 without launching when n == 0. */
+int b200svd_resize_bicubic_u8(const void* x, int64_t n, int h_in, int w_in, void* out, int h_out, int w_out,
+                              const int32_t* bounds_x, const int32_t* taps_x, int kx, const int32_t* bounds_y,
+                              const int32_t* taps_y, int ky, void* workspace, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

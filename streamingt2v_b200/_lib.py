@@ -134,6 +134,7 @@ PROTOTYPES = {
     "b200svd_vfi_merge": [_P, _P, _P, _P, _I64, _I, _I, _P, _P, _P],
     "b200svd_vfi_pair_input": [_P, _P, _I, _I, _P, _P, _P],
     "b200svd_vfi_frames_to_bgr": [_P, _I64, _I, _I, _P, _P],
+    "b200svd_resize_bicubic_u8": [_P, _I64, _I, _I, _P, _I, _I, _P, _P, _I, _P, _P, _I, _P, _P],
 }
 
 

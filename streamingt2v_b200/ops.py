@@ -7,6 +7,7 @@ from __future__ import annotations
 
 import ctypes as C
 import itertools
+import operator
 import os
 from functools import lru_cache
 
@@ -362,7 +363,8 @@ def _conv_common(x, a_dims, a_strides, a_box, w, Cout, K, taps, m_ext, m_box, m_
 _FAMILY = {"b200svd_flash_attn": "flash_attn", "b200svd_flash_attn_d80": "flash_attn",
            "b200svd_clip_preprocess": "clip_preprocess", "b200svd_small_attn": "small_attn", "b200svd_pixel_attn": "pixel_attn", "b200svd_gn_stats": "groupnorm",
            "b200svd_gn_stats_partials": "groupnorm",
-           "b200svd_gn_apply": "groupnorm", "b200svd_layernorm": "layernorm"}
+           "b200svd_gn_apply": "groupnorm", "b200svd_layernorm": "layernorm",
+           "b200svd_resize_bicubic_u8": "resize"}
 
 
 def _call(name, *args, flops=0.0, nbytes=0.0, desc=""):
@@ -871,4 +873,82 @@ def vfi_frames_to_bgr(frames, out=None):
     assert out.is_contiguous() and out.shape == (Fn, 3, H, W) and out.dtype == torch.float32
     _call("b200svd_vfi_frames_to_bgr", _ptr(frames), Fn, H, W, _ptr(out), _stream(), nbytes=15.0 * frames.numel() / 3,
           desc=f"{Fn}x{H}x{W}")
+    return out
+
+
+# ----------------------------------------------------------------------------------------------------------------
+# PIL's BICUBIC resize of uint8 frames
+# ----------------------------------------------------------------------------------------------------------------
+RESIZE_PRECISION_BITS = 22          # Pillow's PRECISION_BITS for 8-bit images
+
+
+def _pil_bicubic(x: float) -> float:
+    """Pillow's bicubic_filter (a = -0.5)."""
+    a = -0.5
+    x = abs(x)
+    if x < 1.0:
+        return ((a + 2.0) * x - (a + 3.0)) * x * x + 1.0
+    if x < 2.0:
+        return (((x - 5.0) * x + 8.0) * x - 4.0) * a
+    return 0.0
+
+
+@lru_cache(maxsize=None)
+def bicubic_taps(in_size: int, out_size: int):
+    """Integer taps of Pillow's 8-bit BICUBIC resize along one axis of in_size -> out_size samples, computed in double
+    precision in Pillow's order (libImaging/Resample.c, precompute_coeffs and normalize_coeffs_8bpc).  Returns CPU
+    int32 tensors: bounds [out_size, 2] = (first source index, tap count) and taps [out_size, k] in 2^-22 units,
+    zero past each tap count.  Cached per size pair; do not modify the result."""
+    scale = in_size / out_size
+    filterscale = max(scale, 1.0)
+    support = 2.0 * filterscale
+    ss = 1.0 / filterscale
+    one = float(1 << RESIZE_PRECISION_BITS)
+    bounds, rows = [], []
+    for xx in range(out_size):
+        center = (xx + 0.5) * scale
+        xmin = max(int(center - support + 0.5), 0)
+        n = min(int(center + support + 0.5), in_size) - xmin
+        w = [_pil_bicubic((x + xmin - center + 0.5) * ss) for x in range(n)]
+        total = 0.0
+        for v in w:                     # left to right, as Pillow does (Python's sum() of floats is compensated)
+            total += v
+        if total != 0.0:
+            w = [v / total for v in w]
+        rows.append([int(v * one - 0.5) if v < 0 else int(v * one + 0.5) for v in w])
+        bounds.append((xmin, n))
+    k = max(len(r) for r in rows)
+    taps = torch.tensor([r + [0] * (k - len(r)) for r in rows], dtype=torch.int32)
+    return torch.tensor(bounds, dtype=torch.int32), taps
+
+
+@lru_cache(maxsize=None)
+def _bicubic_taps_on(in_size: int, out_size: int, device: torch.device):
+    bounds, taps = bicubic_taps(in_size, out_size)
+    return bounds.to(device), taps.to(device)
+
+
+def resize_bicubic_u8(x, W, H):
+    """`PIL.Image.resize((W, H))` with BICUBIC, byte for byte, for a batch of uint8 RGB frames: x uint8 [F, h, w, 3]
+    on a CUDA device -> uint8 [F, H, W, 3] on the same device.  Raises ValueError for any other input."""
+    if not isinstance(x, torch.Tensor) or x.dtype != torch.uint8 or x.dim() != 4 or x.shape[3] != 3 or not x.is_cuda:
+        got = f"{tuple(x.shape)} {x.dtype} on {x.device}" if isinstance(x, torch.Tensor) else type(x).__name__
+        raise ValueError(f"resize_bicubic_u8 takes uint8 [F, H, W, 3] frames on a CUDA device, got {got}")
+    try:
+        W, H = operator.index(W), operator.index(H)
+    except TypeError:
+        raise ValueError(f"resize_bicubic_u8: W and H must be integers, got {W!r}, {H!r}") from None
+    Fn, h, w, _ = x.shape
+    if W < 1 or H < 1 or h < 1 or w < 1:
+        raise ValueError(f"resize_bicubic_u8: sizes must be positive, got {w}x{h} -> {W}x{H}")
+    x = x.contiguous()
+    dev = x.device
+    out = torch.empty((Fn, H, W, 3), dtype=torch.uint8, device=dev)
+    bx, tx = _bicubic_taps_on(w, W, dev) if W != w else (None, None)
+    by, ty = _bicubic_taps_on(h, H, dev) if H != h else (None, None)
+    ws = torch.empty((Fn, h, W, 3), dtype=torch.uint8, device=dev) if (W != w and H != h) else None
+    _call("b200svd_resize_bicubic_u8", _ptr(x), Fn, h, w, _ptr(out), H, W, _ptr(bx), _ptr(tx),
+          0 if tx is None else tx.shape[1], _ptr(by), _ptr(ty), 0 if ty is None else ty.shape[1], _ptr(ws), _stream(),
+          nbytes=float(x.numel() + out.numel() + (2 * ws.numel() if ws is not None else 0)),
+          desc=f"{Fn}x{w}x{h}->{W}x{H}")
     return out
