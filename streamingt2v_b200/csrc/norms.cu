@@ -13,20 +13,100 @@
 namespace b200 {
 
 // ------------------------------------------------------------------------------------------------------------
-// GroupNorm statistics: x [N][P][C] bf16 (row stride ldx) -> sums [N][32][2] (double: sum, sum of squares).
-// grid = (chunks, N); block = (C/8) * rows_per_iter threads; each thread owns one 8-channel vector column.
+// GroupNorm statistics -> sums [N][32][2] (double: sum, sum of squares), deterministic (fixed summation order, no
+// floating-point atomics): every block folds its per-channel fp32 sums into 32 group partials in double and writes
+// them to partial[n][chunk][32][2]; the LAST block of sample n (atomic ticket) adds the chunk partials of the sample
+// in chunk order.  grid = (chunks, N).
 // ------------------------------------------------------------------------------------------------------------
+
+// sm [rstep][2][C]: per-channel sums (sum, then sum of squares) of the block; threads 0-63 each add one group's
+// channels, each channel's rstep copies in order in fp32, then the channels in order in double.
+__device__ __forceinline__ void gn_fold_groups(const float* sm, int C, int rstep, double* __restrict__ partial, int n) {
+  if (threadIdx.x < 64) {
+    const int g = threadIdx.x & 31, which = threadIdx.x >> 5;  // which: 0 = sum, 1 = sum of squares
+    const int cpg = C >> 5;
+    double a = 0.0;
+    for (int j = 0; j < cpg; ++j) {
+      float c = 0.f;
+      for (int r = 0; r < rstep; ++r) c += sm[(size_t)r * 2 * C + which * C + g * cpg + j];
+      a += (double)c;
+    }
+    partial[(((int64_t)n * gridDim.x + blockIdx.x) * 32 + g) * 2 + which] = a;
+  }
+}
+
+// True, in every thread, in the block that finishes sample n last; that block resets the sample's ticket counter
+// for the next launch.
+__device__ __forceinline__ bool gn_last_block(int* __restrict__ counters, int n) {
+  __shared__ int is_last;
+  __threadfence();
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    const int ticket = atomicAdd(&counters[n], 1);
+    is_last = (ticket == (int)gridDim.x - 1);
+    if (is_last) counters[n] = 0;
+  }
+  __syncthreads();
+  if (is_last) __threadfence();
+  return is_last;
+}
+
+// The last block's reduction of sample n's chunk partials into sums[n], spread over the whole block: thread t owns
+// pair t % 64 and the chunks congruent to t / 64 modulo parts = blockDim / 64 (>= 2); the parts are then added in
+// order.  W independent accumulators, folded pairwise, keep W loads in flight per thread (the chain of dependent
+// double adds over up to ~1000 chunk partials, one L2 round trip each, used to dominate the launch for few, large
+// samples); the summation order stays fixed.  dsm: parts * 64 doubles.
+template <int W>
+__device__ __forceinline__ void gn_reduce_chunks(const double* __restrict__ partial, int n, double* dsm,
+                                                 double* __restrict__ sums) {
+  const int chunks = gridDim.x, parts = blockDim.x / 64;
+  const int pr = threadIdx.x % 64, part = threadIdx.x / 64;
+  if (part < parts) {
+    const double* src = partial + (int64_t)n * chunks * 64 + (pr & 31) * 2 + (pr >> 5);
+    double a[W];
+#pragma unroll
+    for (int i = 0; i < W; ++i) a[i] = 0.0;
+    int c = part;
+    for (; c + (W - 1) * parts < chunks; c += W * parts) {
+#pragma unroll
+      for (int i = 0; i < W; ++i) a[i] += src[(int64_t)(c + i * parts) * 64];
+    }
+    for (; c < chunks; c += parts) a[0] += src[(int64_t)c * 64];
+#pragma unroll
+    for (int w = W / 2; w > 0; w >>= 1)
+#pragma unroll
+      for (int i = 0; i < w; ++i) a[i] += a[i + w];
+    dsm[part * 64 + pr] = a[0];
+  }
+  __syncthreads();
+  if (threadIdx.x < 64) {
+    double a = 0.0;
+    for (int q = 0; q < parts; ++q) a += dsm[q * 64 + threadIdx.x];
+    sums[((int64_t)n * 32 + (threadIdx.x & 31)) * 2 + (threadIdx.x >> 5)] = a;
+  }
+}
+
+// Calls f(p, u) for the rows p, p + rstep, ... below p1, u the 16 bytes at row p of xb; 4 loads in flight per thread.
+template <class F>
+__device__ __forceinline__ void gn_for_rows(const __nv_bfloat16* xb, int64_t ldx, int p, int p1, int rstep, F&& f) {
+  constexpr int U = 4;
+  for (; p + (U - 1) * rstep < p1; p += U * rstep) {
+    uint4 u[U];
+#pragma unroll
+    for (int i = 0; i < U; ++i) u[i] = __ldg(reinterpret_cast<const uint4*>(xb + (int64_t)(p + i * rstep) * ldx));
+#pragma unroll
+    for (int i = 0; i < U; ++i) f(p + i * rstep, u[i]);
+  }
+  for (; p < p1; p += rstep) f(p, __ldg(reinterpret_cast<const uint4*>(xb + (int64_t)p * ldx)));
+}
+
+// x [N][P][C] bf16 (row stride ldx).  block = (C/8) * rows_per_iter threads; each thread owns one 8-channel vector
+// column: thread partials -> smem [rstep][2][C] -> gn_fold_groups.
 __global__ void gn_stats_kernel(const __nv_bfloat16* __restrict__ x, int64_t ldx, int P, int C, int rows_per_chunk,
                                 double* __restrict__ sums, double* __restrict__ partial, int* __restrict__ counters) {
-  // Deterministic (fixed summation order, no floating-point atomics):
-  //   thread partials -> smem [rstep][2C] -> per-channel sums (fixed order over rstep) -> per-group chunk partial
-  //   (double) -> global partial[n][chunk][64]; the LAST chunk block of sample n (atomic ticket) adds all chunk
-  //   partials in chunk order and writes sums[n][32][2].
-  extern __shared__ float sm[];  // [rstep][2][C]
-  __shared__ int is_last;
+  extern __shared__ float sm[];  // [rstep][2][C]; the last block reuses it for blockDim / 64 * 64 doubles
   const int vecs = C >> 3;
   const int n = blockIdx.y;
-  const int chunks = gridDim.x;
   const int p0 = blockIdx.x * rows_per_chunk;
   const int p1 = min(P, p0 + rows_per_chunk);
   const int v = threadIdx.x % vecs;
@@ -35,28 +115,7 @@ __global__ void gn_stats_kernel(const __nv_bfloat16* __restrict__ x, int64_t ldx
   float s[8], q[8];
 #pragma unroll
   for (int j = 0; j < 8; ++j) s[j] = q[j] = 0.f;
-  const __nv_bfloat16* base = x + ((int64_t)n * P) * ldx + v * 8;
-  constexpr int U = 4;  // independent 16-byte loads in flight per thread
-  int p = p0 + r0;
-  for (; p + (U - 1) * rstep < p1; p += U * rstep) {
-    uint4 u[U];
-#pragma unroll
-    for (int i = 0; i < U; ++i) u[i] = __ldg(reinterpret_cast<const uint4*>(base + (int64_t)(p + i * rstep) * ldx));
-#pragma unroll
-    for (int i = 0; i < U; ++i) {
-      const uint32_t w[4] = {u[i].x, u[i].y, u[i].z, u[i].w};
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const float a = bf16_lo(w[j]), b = bf16_hi(w[j]);
-        s[2 * j] += a;
-        q[2 * j] += a * a;
-        s[2 * j + 1] += b;
-        q[2 * j + 1] += b * b;
-      }
-    }
-  }
-  for (; p < p1; p += rstep) {
-    const uint4 u = __ldg(reinterpret_cast<const uint4*>(base + (int64_t)p * ldx));
+  gn_for_rows(x + ((int64_t)n * P) * ldx + v * 8, ldx, p0 + r0, p1, rstep, [&](int, const uint4& u) {
     const uint32_t w[4] = {u.x, u.y, u.z, u.w};
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
@@ -66,7 +125,7 @@ __global__ void gn_stats_kernel(const __nv_bfloat16* __restrict__ x, int64_t ldx
       s[2 * j + 1] += b;
       q[2 * j + 1] += b * b;
     }
-  }
+  });
   float* mine = sm + (size_t)r0 * 2 * C;
 #pragma unroll
   for (int j = 0; j < 8; ++j) {
@@ -74,80 +133,22 @@ __global__ void gn_stats_kernel(const __nv_bfloat16* __restrict__ x, int64_t ldx
     mine[C + v * 8 + j] = q[j];
   }
   __syncthreads();
-  const int cpg = C >> 5;
-  if (threadIdx.x < 64) {
-    const int g = threadIdx.x & 31, which = threadIdx.x >> 5;  // which: 0 = sum, 1 = sum of squares
-    double a = 0.0;
-    for (int j = 0; j < cpg; ++j) {
-      float c = 0.f;
-      for (int r = 0; r < rstep; ++r) c += sm[(size_t)r * 2 * C + which * C + g * cpg + j];
-      a += (double)c;
-    }
-    partial[(((int64_t)n * chunks + blockIdx.x) * 32 + g) * 2 + which] = a;
-  }
-  __threadfence();
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    const int ticket = atomicAdd(&counters[n], 1);
-    is_last = (ticket == chunks - 1);
-    if (is_last) counters[n] = 0;  // self-reset for the next launch
-  }
-  __syncthreads();
-  if (is_last) {
-    // fixed-order final reduction over the chunk partials, spread over the whole block: thread t owns pair t%64 and
-    // the chunks congruent to t/64 modulo (blockDim/64); the (blockDim/64) strided sums are then added in order
-    __threadfence();
-    const int pairs = 64;
-    const int parts = blockDim.x / pairs;  // >= 2 (blockDim >= 160)
-    double* dsm = reinterpret_cast<double*>(sm);  // reuse the staging area: needs parts*64 doubles <= 2*C*rstep floats
-    const int pr = threadIdx.x % pairs, part = threadIdx.x / pairs;
-    if (part < parts) {
-      // 16 independent partial sums keep 16 loads in flight per thread (the chain of dependent double adds over up
-      // to ~1000 chunk partials, one L2 round trip each, used to dominate the launch for few, large samples); the
-      // summation order stays fixed
-      const double* src = partial + (int64_t)n * chunks * 64 + (pr & 31) * 2 + (pr >> 5);
-      constexpr int W = 16;
-      double a[W];
-#pragma unroll
-      for (int i = 0; i < W; ++i) a[i] = 0.0;
-      int c = part;
-      for (; c + (W - 1) * parts < chunks; c += W * parts) {
-#pragma unroll
-        for (int i = 0; i < W; ++i) a[i] += src[(int64_t)(c + i * parts) * 64];
-      }
-      for (; c < chunks; c += parts) a[0] += src[(int64_t)c * 64];
-#pragma unroll
-      for (int w = W / 2; w > 0; w >>= 1)
-#pragma unroll
-        for (int i = 0; i < w; ++i) a[i] += a[i + w];
-      dsm[part * pairs + pr] = a[0];
-    }
-    __syncthreads();
-    if (threadIdx.x < pairs) {
-      double a = 0.0;
-      for (int q = 0; q < parts; ++q) a += dsm[q * pairs + threadIdx.x];
-      sums[((int64_t)n * 32 + (threadIdx.x & 31)) * 2 + (threadIdx.x >> 5)] = a;
-    }
-  }
+  gn_fold_groups(sm, C, rstep, partial, n);
+  if (gn_last_block(counters, n)) gn_reduce_chunks<16>(partial, n, reinterpret_cast<double*>(sm), sums);
 }
 
-// ------------------------------------------------------------------------------------------------------------
-// GroupNorm statistics from the per-quadrant partials written by the GEMM epilogue (mtgemm.cu, gn_part):
-// part [n_slots][ld][2] fp32 (sum, sum of squares per channel over the <= 32 rows of a slot), slot_sample [n_slots].
-// grid = (chunks of 64 slots, N); the block adds the slots of ITS sample in slot order (fixed), folds channels into
-// groups in double, and the last block of the sample (ticket) adds the chunk partials in chunk order: deterministic.
-// ------------------------------------------------------------------------------------------------------------
+// From the per-quadrant partials written by the GEMM epilogue (mtgemm.cu, gn_part): part [n_slots][ld][2] fp32 (sum,
+// sum of squares per channel over the <= 32 rows of a slot), slot_sample [n_slots].  A block takes 64 slots and adds
+// those of ITS sample in slot order.
 constexpr int GNP_SLOTS = 64;
 constexpr int GNP_THREADS = 256;
 __global__ void __launch_bounds__(GNP_THREADS)
 gn_stats_partials_kernel(const float2* __restrict__ part, const int* __restrict__ slot_sample, int64_t n_slots,
                          int64_t ld, int C, double* __restrict__ sums, double* __restrict__ partial,
                          int* __restrict__ counters) {
-  extern __shared__ float sm[];  // [2][C], reused as doubles by the last block
-  __shared__ int is_last;
+  extern __shared__ float sm[];  // [2][C]; the last block reuses it for 4 * 64 doubles (C >= 256: checked on host)
   __shared__ int hit[GNP_SLOTS];
   const int n = blockIdx.y;
-  const int chunks = gridDim.x;
   const int64_t s0 = (int64_t)blockIdx.x * GNP_SLOTS;
   if (threadIdx.x < GNP_SLOTS) {
     const int64_t sl = s0 + threadIdx.x;
@@ -167,51 +168,8 @@ gn_stats_partials_kernel(const float2* __restrict__ part, const int* __restrict_
     sm[C + c] = b;
   }
   __syncthreads();
-  const int cpg = C >> 5;
-  if (threadIdx.x < 64) {
-    const int g = threadIdx.x & 31, which = threadIdx.x >> 5;
-    double a = 0.0;
-    for (int j = 0; j < cpg; ++j) a += (double)sm[which * C + g * cpg + j];
-    partial[(((int64_t)n * chunks + blockIdx.x) * 32 + g) * 2 + which] = a;
-  }
-  __threadfence();
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    const int ticket = atomicAdd(&counters[n], 1);
-    is_last = (ticket == chunks - 1);
-    if (is_last) counters[n] = 0;
-  }
-  __syncthreads();
-  if (is_last) {
-    __threadfence();
-    const int pairs = 64;
-    const int parts = GNP_THREADS / pairs;  // 4
-    double* dsm = reinterpret_cast<double*>(sm);  // parts * 64 doubles = 2 KB <= 2 * C floats (C >= 256) — checked on host
-    const int pr = threadIdx.x % pairs, part_i = threadIdx.x / pairs;
-    const double* src = partial + (int64_t)n * chunks * 64 + (pr & 31) * 2 + (pr >> 5);
-    constexpr int W = 8;
-    double a[W];
-#pragma unroll
-    for (int i = 0; i < W; ++i) a[i] = 0.0;
-    int c = part_i;
-    for (; c + (W - 1) * parts < chunks; c += W * parts) {
-#pragma unroll
-      for (int i = 0; i < W; ++i) a[i] += src[(int64_t)(c + i * parts) * 64];
-    }
-    for (; c < chunks; c += parts) a[0] += src[(int64_t)c * 64];
-#pragma unroll
-    for (int w = W / 2; w > 0; w >>= 1)
-#pragma unroll
-      for (int i = 0; i < w; ++i) a[i] += a[i + w];
-    __syncthreads();
-    dsm[part_i * pairs + pr] = a[0];
-    __syncthreads();
-    if (threadIdx.x < pairs) {
-      double t = 0.0;
-      for (int q = 0; q < parts; ++q) t += dsm[q * pairs + threadIdx.x];
-      sums[((int64_t)n * 32 + (threadIdx.x & 31)) * 2 + (threadIdx.x >> 5)] = t;
-    }
-  }
+  gn_fold_groups(sm, C, 1, partial, n);
+  if (gn_last_block(counters, n)) gn_reduce_chunks<8>(partial, n, reinterpret_cast<double*>(sm), sums);
 }
 
 // y = [silu]((x - mean) * rstd * gamma + beta), bf16 out (row stride ldy).
@@ -248,9 +206,8 @@ __global__ void gn_apply_kernel(const __nv_bfloat16* __restrict__ x, int64_t ldx
     sc[j] = rstd * ga;
     sh[j] = be - mean_f * rstd * ga;
   }
-  const __nv_bfloat16* xb = x + ((int64_t)n * P) * ldx + v * 8;
   __nv_bfloat16* yb = y + ((int64_t)n * P) * ldy + v * 8;
-  auto apply8 = [&](const uint4& u) {
+  gn_for_rows(x + ((int64_t)n * P) * ldx + v * 8, ldx, p0 + r0, p1, rstep, [&](int p, const uint4& u) {
     const uint32_t w[4] = {u.x, u.y, u.z, u.w};
     uint32_t o[4];
 #pragma unroll
@@ -263,248 +220,118 @@ __global__ void gn_apply_kernel(const __nv_bfloat16* __restrict__ x, int64_t ldx
       }
       o[j] = pack_bf16x2(a, b);
     }
-    return make_uint4(o[0], o[1], o[2], o[3]);
-  };
-  constexpr int U = 4;
-  int p = p0 + r0;
-  for (; p + (U - 1) * rstep < p1; p += U * rstep) {
-    uint4 u[U];
-#pragma unroll
-    for (int i = 0; i < U; ++i) u[i] = __ldg(reinterpret_cast<const uint4*>(xb + (int64_t)(p + i * rstep) * ldx));
-#pragma unroll
-    for (int i = 0; i < U; ++i) *reinterpret_cast<uint4*>(yb + (int64_t)(p + i * rstep) * ldy) = apply8(u[i]);
-  }
-  for (; p < p1; p += rstep)
-    *reinterpret_cast<uint4*>(yb + (int64_t)p * ldy) = apply8(__ldg(reinterpret_cast<const uint4*>(xb + (int64_t)p * ldx)));
+    *reinterpret_cast<uint4*>(yb + (int64_t)p * ldy) = make_uint4(o[0], o[1], o[2], o[3]);
+  });
 }
 
 // ------------------------------------------------------------------------------------------------------------
-// LayerNorm over the channel dim: one warp per row.  y = ((x [+ fvec[row/rpf]]) - mean) * rstd * gamma + beta
-// Optional: also write xsum = x + fvec (bf16) so the caller can use it as the residual stream, and fused SiLU.
+// LayerNorm over the channel dim, fp32 two-pass statistics:  y = [silu](((x [+ fvec[row/rpf]]) - mean) * rstd * gamma
+// + beta).  With xsum, also writes xsum = bf16(x + fvec), which the caller uses as the residual stream, and normalises
+// that rounded sum.  LPR lanes own one row (32 / LPR rows per warp), lane li its 16-byte vectors li + i * LPR for
+// i < V; vectors past C/8 are skipped.  VEC: gamma, beta and fvec are 16-byte aligned and load as float4 pairs, else
+// one float at a time.
 // ------------------------------------------------------------------------------------------------------------
-template <int MAXV>  // max 8-channel vectors per lane
-__global__ void layernorm_kernel(const __nv_bfloat16* __restrict__ x, int64_t ldx, __nv_bfloat16* __restrict__ y,
-                                 int64_t ldy, int64_t rows, int C, const float* __restrict__ gamma,
-                                 const float* __restrict__ beta, float eps, const float* __restrict__ fvec, int64_t ldf,
-                                 int rows_per_frame, __nv_bfloat16* __restrict__ xsum, int64_t ldxs, int apply_silu) {
-  const int lane = threadIdx.x & 31;
-  const int64_t row = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-  if (row >= rows) return;
-  const int vecs = C >> 3;
-  float val[MAXV][8];
-  const __nv_bfloat16* xr = x + row * ldx;
-  const float* fr = fvec ? fvec + (row / rows_per_frame) * ldf : nullptr;
-  float sum = 0.f;
-#pragma unroll
-  for (int i = 0; i < MAXV; ++i) {
-    const int v = lane + i * 32;
-    if (v < vecs) {
-      const uint4 u = __ldg(reinterpret_cast<const uint4*>(xr + v * 8));
-      const uint32_t w[4] = {u.x, u.y, u.z, u.w};
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        val[i][2 * j] = bf16_lo(w[j]);
-        val[i][2 * j + 1] = bf16_hi(w[j]);
-      }
-      if (fr) {
-#pragma unroll
-        for (int j = 0; j < 8; ++j) val[i][j] += __ldg(fr + v * 8 + j);
-        if (xsum) {
-          uint32_t o[4];
-#pragma unroll
-          for (int j = 0; j < 4; ++j) o[j] = pack_bf16x2(val[i][2 * j], val[i][2 * j + 1]);
-          *reinterpret_cast<uint4*>(xsum + row * ldxs + v * 8) = make_uint4(o[0], o[1], o[2], o[3]);
-          // the residual stream is the bf16-rounded sum; normalise exactly what the consumer will see
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            val[i][2 * j] = bf16_lo(o[j]);
-            val[i][2 * j + 1] = bf16_hi(o[j]);
-          }
-        }
-      }
-#pragma unroll
-      for (int j = 0; j < 8; ++j) sum += val[i][j];
-    }
-  }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
-  const float mean = sum / (float)C;
-  float sq = 0.f;
-#pragma unroll
-  for (int i = 0; i < MAXV; ++i) {
-    const int v = lane + i * 32;
-    if (v < vecs) {
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const float d = val[i][j] - mean;
-        sq += d * d;
-      }
-    }
-  }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) sq += __shfl_xor_sync(0xffffffffu, sq, o);
-  const float rstd = rsqrtf(sq / (float)C + eps);
-  __nv_bfloat16* yr = y + row * ldy;
-#pragma unroll
-  for (int i = 0; i < MAXV; ++i) {
-    const int v = lane + i * 32;
-    if (v < vecs) {
-      float o8[8];
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const int c = v * 8 + j;
-        float t = (val[i][j] - mean) * rstd * __ldg(gamma + c) + __ldg(beta + c);
-        if (apply_silu) t = silu_fast(t);
-        o8[j] = t;
-      }
-      *reinterpret_cast<uint4*>(yr + v * 8) = make_uint4(pack_bf16x2(o8[0], o8[1]), pack_bf16x2(o8[2], o8[3]),
-                                                          pack_bf16x2(o8[4], o8[5]), pack_bf16x2(o8[6], o8[7]));
-    }
-  }
+__device__ __forceinline__ void load8(const float* __restrict__ p, float (&o)[8]) {
+  const float4 a = __ldg(reinterpret_cast<const float4*>(p)), b = __ldg(reinterpret_cast<const float4*>(p) + 1);
+  o[0] = a.x; o[1] = a.y; o[2] = a.z; o[3] = a.w;
+  o[4] = b.x; o[5] = b.y; o[6] = b.z; o[7] = b.w;
 }
 
-// Narrow rows (C <= 256: the ControlNet condition-embedding norms): LPR lanes own one row, one 16-byte vector each
-// (lanes >= C/8 idle), 32/LPR rows per warp, so a warp issues full-width loads instead of one 64-byte row at a time.
-template <int LPR>
-__global__ void __launch_bounds__(256) layernorm_narrow_kernel(
-    const __nv_bfloat16* __restrict__ x, int64_t ldx, __nv_bfloat16* __restrict__ y, int64_t ldy, int64_t rows, int C,
-    const float* __restrict__ gamma, const float* __restrict__ beta, float eps, int apply_silu) {
-  constexpr int RPW = 32 / LPR;
-  const int lane = threadIdx.x & 31;
-  const int sub = lane / LPR, li = lane % LPR;
-  const int64_t row = ((int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5)) * RPW + sub;
-  const bool active = row < rows && li < (C >> 3);
-  float val[8];
-#pragma unroll
-  for (int j = 0; j < 8; ++j) val[j] = 0.f;
-  if (active) {
-    const uint4 u = __ldg(reinterpret_cast<const uint4*>(x + row * ldx + li * 8));
-    const uint32_t w[4] = {u.x, u.y, u.z, u.w};
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      val[2 * j] = bf16_lo(w[j]);
-      val[2 * j + 1] = bf16_hi(w[j]);
-    }
-  }
-  float sum = 0.f;
-#pragma unroll
-  for (int j = 0; j < 8; ++j) sum += val[j];
-#pragma unroll
-  for (int o = LPR / 2; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
-  const float mean = sum / (float)C;
-  float sq = 0.f;
-  if (active) {
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const float d = val[j] - mean;
-      sq += d * d;
-    }
-  }
-#pragma unroll
-  for (int o = LPR / 2; o > 0; o >>= 1) sq += __shfl_xor_sync(0xffffffffu, sq, o);
-  const float rstd = rsqrtf(sq / (float)C + eps);
-  if (!active) return;
-  const int c0 = li * 8;
-  const float4 g0 = __ldg(reinterpret_cast<const float4*>(gamma + c0)), g1 = __ldg(reinterpret_cast<const float4*>(gamma + c0) + 1);
-  const float4 b0 = __ldg(reinterpret_cast<const float4*>(beta + c0)), b1 = __ldg(reinterpret_cast<const float4*>(beta + c0) + 1);
-  const float gg[8] = {g0.x, g0.y, g0.z, g0.w, g1.x, g1.y, g1.z, g1.w};
-  const float bb[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
-  float o8[8];
-#pragma unroll
-  for (int j = 0; j < 8; ++j) {
-    float t = (val[j] - mean) * rstd * gg[j] + bb[j];
-    if (apply_silu) t = silu_fast(t);
-    o8[j] = t;
-  }
-  *reinterpret_cast<uint4*>(y + row * ldy + c0) = make_uint4(pack_bf16x2(o8[0], o8[1]), pack_bf16x2(o8[2], o8[3]),
-                                                             pack_bf16x2(o8[4], o8[5]), pack_bf16x2(o8[6], o8[7]));
-}
-
-// Fast path for C = 40*LPR channels-vectors (C = 320, 640, 1280): LPR lanes own one row, 5 x 16-byte vectors each,
-// all loads issued before first use; 32/LPR rows per warp.
-template <int LPR>
-__global__ void __launch_bounds__(256) layernorm5_kernel(
+template <int LPR, int V, bool VEC>
+__global__ void __launch_bounds__(256) layernorm_kernel(
     const __nv_bfloat16* __restrict__ x, int64_t ldx, __nv_bfloat16* __restrict__ y, int64_t ldy, int64_t rows, int C,
     const float* __restrict__ gamma, const float* __restrict__ beta, float eps, const float* __restrict__ fvec,
     int64_t ldf, int rows_per_frame, __nv_bfloat16* __restrict__ xsum, int64_t ldxs, int apply_silu) {
-  constexpr int RPW = 32 / LPR;
-  const int lane = threadIdx.x & 31;
-  const int sub = lane / LPR, li = lane % LPR;
-  const int64_t row = ((int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5)) * RPW + sub;
+  const int lane = threadIdx.x & 31, li = lane % LPR;
+  const int64_t row = ((int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5)) * (32 / LPR) + lane / LPR;
+  if (LPR == 32 && row >= rows) return;
+  // a row past the end (LPR < 32) stores nothing, but reads the last row so that its lanes still take part in their
+  // warp's shuffles
   const bool active = row < rows;
   const int64_t rr = active ? row : rows - 1;
+  // V = 5 runs only at C = 40 LPR: every vector is owned, and the constant lets the compiler drop the checks
+  const int vecs = V == 5 ? 5 * LPR : C >> 3;
+  auto own = [&](int i) { return li + i * LPR < vecs; };
   const __nv_bfloat16* xr = x + rr * ldx;
-  uint4 u[5];
+  const float* fr = fvec ? fvec + (rr / rows_per_frame) * ldf : nullptr;
+  uint4 u[V];  // every load issued before the first use
 #pragma unroll
-  for (int i = 0; i < 5; ++i) u[i] = __ldg(reinterpret_cast<const uint4*>(xr + (li + i * LPR) * 8));
-  float val[5][8];
+  for (int i = 0; i < V; ++i)
+    if (own(i)) u[i] = __ldg(reinterpret_cast<const uint4*>(xr + (li + i * LPR) * 8));
+  float val[V][8];
 #pragma unroll
-  for (int i = 0; i < 5; ++i) {
+  for (int i = 0; i < V; ++i) {
+    if (!own(i)) continue;
+    const int c0 = (li + i * LPR) * 8;
     const uint32_t w[4] = {u[i].x, u[i].y, u[i].z, u[i].w};
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
       val[i][2 * j] = bf16_lo(w[j]);
       val[i][2 * j + 1] = bf16_hi(w[j]);
     }
+    if (fr) {
+      float f[8];
+      if constexpr (VEC) load8(fr + c0, f);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) val[i][j] += VEC ? f[j] : __ldg(fr + c0 + j);
+    }
   }
-  if (fvec != nullptr) {
-    const float* fr = fvec + (rr / rows_per_frame) * ldf;
+  if (fr && xsum) {
+    // every per-frame load is issued before the first store
 #pragma unroll
-    for (int i = 0; i < 5; ++i) {
-      const float4 f0 = __ldg(reinterpret_cast<const float4*>(fr + (li + i * LPR) * 8));
-      const float4 f1 = __ldg(reinterpret_cast<const float4*>(fr + (li + i * LPR) * 8) + 1);
-      val[i][0] += f0.x; val[i][1] += f0.y; val[i][2] += f0.z; val[i][3] += f0.w;
-      val[i][4] += f1.x; val[i][5] += f1.y; val[i][6] += f1.z; val[i][7] += f1.w;
-      if (xsum != nullptr) {
-        uint32_t o[4];
+    for (int i = 0; i < V; ++i) {
+      if (!active || !own(i)) continue;
+      uint32_t o[4];
 #pragma unroll
-        for (int j = 0; j < 4; ++j) o[j] = pack_bf16x2(val[i][2 * j], val[i][2 * j + 1]);
-        if (active) *reinterpret_cast<uint4*>(xsum + row * ldxs + (li + i * LPR) * 8) = make_uint4(o[0], o[1], o[2], o[3]);
+      for (int j = 0; j < 4; ++j) o[j] = pack_bf16x2(val[i][2 * j], val[i][2 * j + 1]);
+      *reinterpret_cast<uint4*>(xsum + row * ldxs + (li + i * LPR) * 8) = make_uint4(o[0], o[1], o[2], o[3]);
+      // the residual stream is the bf16-rounded sum; normalise exactly what the consumer will see
 #pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          val[i][2 * j] = bf16_lo(o[j]);
-          val[i][2 * j + 1] = bf16_hi(o[j]);
-        }
+      for (int j = 0; j < 4; ++j) {
+        val[i][2 * j] = bf16_lo(o[j]);
+        val[i][2 * j + 1] = bf16_hi(o[j]);
       }
     }
   }
   float sum = 0.f;
 #pragma unroll
-  for (int i = 0; i < 5; ++i)
+  for (int i = 0; i < V; ++i)
+    if (own(i))
 #pragma unroll
-    for (int j = 0; j < 8; ++j) sum += val[i][j];
+      for (int j = 0; j < 8; ++j) sum += val[i][j];
 #pragma unroll
   for (int o = LPR / 2; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
   const float mean = sum / (float)C;
   float sq = 0.f;
 #pragma unroll
-  for (int i = 0; i < 5; ++i)
+  for (int i = 0; i < V; ++i)
+    if (own(i))
 #pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const float d = val[i][j] - mean;
-      sq += d * d;
-    }
+      for (int j = 0; j < 8; ++j) {
+        const float d = val[i][j] - mean;
+        sq += d * d;
+      }
 #pragma unroll
   for (int o = LPR / 2; o > 0; o >>= 1) sq += __shfl_xor_sync(0xffffffffu, sq, o);
   const float rstd = rsqrtf(sq / (float)C + eps);
-  if (!active) return;
   __nv_bfloat16* yr = y + row * ldy;
 #pragma unroll
-  for (int i = 0; i < 5; ++i) {
+  for (int i = 0; i < V; ++i) {
+    if (!active || !own(i)) continue;
     const int c0 = (li + i * LPR) * 8;
-    const float4 g0 = __ldg(reinterpret_cast<const float4*>(gamma + c0)), g1 = __ldg(reinterpret_cast<const float4*>(gamma + c0) + 1);
-    const float4 b0 = __ldg(reinterpret_cast<const float4*>(beta + c0)), b1 = __ldg(reinterpret_cast<const float4*>(beta + c0) + 1);
-    const float gg[8] = {g0.x, g0.y, g0.z, g0.w, g1.x, g1.y, g1.z, g1.w};
-    const float bb[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
-    float o8[8];
+    float g[8], b[8], o8[8];
+    if constexpr (VEC) {
+      load8(gamma + c0, g);
+      load8(beta + c0, b);
+    }
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
-      float t = (val[i][j] - mean) * rstd * gg[j] + bb[j];
+      float t = (val[i][j] - mean) * rstd * (VEC ? g[j] : __ldg(gamma + c0 + j)) + (VEC ? b[j] : __ldg(beta + c0 + j));
       if (apply_silu) t = silu_fast(t);
       o8[j] = t;
     }
     *reinterpret_cast<uint4*>(yr + c0) = make_uint4(pack_bf16x2(o8[0], o8[1]), pack_bf16x2(o8[2], o8[3]),
-                                                     pack_bf16x2(o8[4], o8[5]), pack_bf16x2(o8[6], o8[7]));
+                                                    pack_bf16x2(o8[4], o8[5]), pack_bf16x2(o8[6], o8[7]));
   }
 }
 
@@ -545,6 +372,22 @@ static int gn_check_shape(const char* who, int64_t n, int64_t p, int c) {
   return 0;
 }
 
+// Lets kernel K take smem bytes of dynamic shared memory: past the default 48 KB the limit is raised, per device, to
+// the largest size asked for so far.
+template <auto K>
+static int allow_dynamic_smem(size_t smem, const char* what) {
+  static size_t smem_set_dev[B200_MAX_DEVICES] = {};
+  size_t& smem_set = smem_set_dev[dev_slot()];
+  if (smem > 48 * 1024 && smem > smem_set) {
+    cudaError_t e = cudaFuncSetAttribute(K, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return cuda_fail(e, what);
+    smem_set = smem;
+  }
+  return 0;
+}
+
+using LayerNormKernel = decltype(&layernorm_kernel<32, 1, false>);
+
 }  // namespace b200
 
 extern "C" {
@@ -571,13 +414,7 @@ int b200svd_gn_stats_partials(const float* gn_part, const int32_t* gn_slot_sampl
   const int64_t chunks = (n_slots + GNP_SLOTS - 1) / GNP_SLOTS;
   dim3 grid((unsigned)chunks, (unsigned)n);
   const size_t smem = (size_t)2 * c * sizeof(float);
-  static size_t smem_set_dev[B200_MAX_DEVICES] = {};
-  size_t& smem_set = smem_set_dev[dev_slot()];
-  if (smem > 48 * 1024 && smem > smem_set) {
-    cudaError_t e = cudaFuncSetAttribute(gn_stats_partials_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(gn_stats_partials)");
-    smem_set = smem;
-  }
+  if (allow_dynamic_smem<gn_stats_partials_kernel>(smem, "cudaFuncSetAttribute(gn_stats_partials)")) return 1;
   gn_stats_partials_kernel<<<grid, GNP_THREADS, smem, reinterpret_cast<cudaStream_t>(stream)>>>(
       reinterpret_cast<const float2*>(gn_part), gn_slot_sample, n_slots, gn_ld, c, reinterpret_cast<double*>(sums),
       reinterpret_cast<double*>(scratch), reinterpret_cast<int*>(counters));
@@ -607,13 +444,7 @@ int b200svd_gn_stats(const void* x, int64_t ldx, int64_t n, int64_t p, int c, vo
   dim3 grid(chunks, (unsigned)n);
   const int rstep = threads / (c / 8);
   const size_t smem = (size_t)rstep * 2 * c * sizeof(float);
-  static size_t smem_set_dev[B200_MAX_DEVICES] = {};
-  size_t& smem_set = smem_set_dev[dev_slot()];
-  if (smem > 48 * 1024 && smem > smem_set) {
-    cudaError_t e = cudaFuncSetAttribute(gn_stats_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return cuda_fail(e, "gn_stats smem attribute");
-    smem_set = smem;
-  }
+  if (allow_dynamic_smem<gn_stats_kernel>(smem, "gn_stats smem attribute")) return 1;
   gn_stats_kernel<<<grid, threads, smem, st>>>(reinterpret_cast<const __nv_bfloat16*>(x), ldx, (int)p, c, rpc,
                                              reinterpret_cast<double*>(sums), reinterpret_cast<double*>(scratch),
                                              reinterpret_cast<int*>(counters));
@@ -685,53 +516,42 @@ int b200svd_layernorm(const void* x, int64_t ldx, void* y, int64_t ldy, int64_t 
     set_error("layernorm: x, y and xsum must be 16-byte aligned");
     return 1;
   }
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  const int wpb = 8;
-  const unsigned grid = (unsigned)((rows + wpb - 1) / wpb);
-  const int vecs = c / 8;
-  const __nv_bfloat16* xp = reinterpret_cast<const __nv_bfloat16*>(x);
-  __nv_bfloat16* yp = reinterpret_cast<__nv_bfloat16*>(y);
-  __nv_bfloat16* xs = reinterpret_cast<__nv_bfloat16*>(xsum);
   if (rows_per_frame <= 0) rows_per_frame = 1;
+  const int vecs = c / 8;
   const bool f_ok = (fvec == nullptr) || (ldf % 4 == 0 && (reinterpret_cast<uintptr_t>(fvec) & 15) == 0);
   const bool gb_ok = ((reinterpret_cast<uintptr_t>(gamma) | reinterpret_cast<uintptr_t>(beta)) & 15) == 0;
-  if ((c == 320 || c == 640 || c == 1280) && f_ok && gb_ok) {
-    const int lpr = c / 40;
-    const int rpw = 32 / lpr;
-    const unsigned g5 = (unsigned)((rows + (int64_t)wpb * rpw - 1) / ((int64_t)wpb * rpw));
-    if (lpr == 8)
-      layernorm5_kernel<8><<<g5, wpb * 32, 0, st>>>(xp, ldx, yp, ldy, rows, c, gamma, beta, eps, fvec, ldf, rows_per_frame, xs, ldxs, apply_silu);
-    else if (lpr == 16)
-      layernorm5_kernel<16><<<g5, wpb * 32, 0, st>>>(xp, ldx, yp, ldy, rows, c, gamma, beta, eps, fvec, ldf, rows_per_frame, xs, ldxs, apply_silu);
-    else
-      layernorm5_kernel<32><<<g5, wpb * 32, 0, st>>>(xp, ldx, yp, ldy, rows, c, gamma, beta, eps, fvec, ldf, rows_per_frame, xs, ldxs, apply_silu);
-    B200_CHECK_LAUNCH("layernorm5");
-    return 0;
+  // layernorm_kernel<lanes per row, vectors per lane, float4 parameter loads>
+  LayerNormKernel kernel;
+  int lpr;
+  const char* name;
+  if ((c == 320 || c == 640 || c == 1280) && f_ok && gb_ok) {  // C = 40 * LPR: 5 vectors per lane, no idle lanes
+    lpr = c / 40;
+    kernel = lpr == 8 ? layernorm_kernel<8, 5, true> : lpr == 16 ? layernorm_kernel<16, 5, true>
+                                                                 : layernorm_kernel<32, 5, true>;
+    name = "layernorm5";
+  } else if (vecs <= 32 && fvec == nullptr && xsum == nullptr && gb_ok) {
+    // narrow rows (C <= 256: the ControlNet condition-embedding norms): a warp issues full-width loads for several rows
+    lpr = vecs <= 4 ? 4 : vecs <= 8 ? 8 : vecs <= 16 ? 16 : 32;
+    kernel = lpr == 4    ? layernorm_kernel<4, 1, true>
+             : lpr == 8  ? layernorm_kernel<8, 1, true>
+             : lpr == 16 ? layernorm_kernel<16, 1, true>
+                         : layernorm_kernel<32, 1, true>;
+    name = "layernorm_narrow";
+  } else {
+    lpr = 32;
+    kernel = vecs <= 32    ? layernorm_kernel<32, 1, false>
+             : vecs <= 64  ? layernorm_kernel<32, 2, false>
+             : vecs <= 128 ? layernorm_kernel<32, 4, false>
+                           : layernorm_kernel<32, 8, false>;
+    name = "layernorm";
   }
-  if (vecs <= 32 && fvec == nullptr && xsum == nullptr && gb_ok) {
-    const int lpr = vecs <= 4 ? 4 : vecs <= 8 ? 8 : vecs <= 16 ? 16 : 32;
-    const int rpw = 32 / lpr;
-    const unsigned gn = (unsigned)((rows + (int64_t)wpb * rpw - 1) / ((int64_t)wpb * rpw));
-    if (lpr == 4)
-      layernorm_narrow_kernel<4><<<gn, wpb * 32, 0, st>>>(xp, ldx, yp, ldy, rows, c, gamma, beta, eps, apply_silu);
-    else if (lpr == 8)
-      layernorm_narrow_kernel<8><<<gn, wpb * 32, 0, st>>>(xp, ldx, yp, ldy, rows, c, gamma, beta, eps, apply_silu);
-    else if (lpr == 16)
-      layernorm_narrow_kernel<16><<<gn, wpb * 32, 0, st>>>(xp, ldx, yp, ldy, rows, c, gamma, beta, eps, apply_silu);
-    else
-      layernorm_narrow_kernel<32><<<gn, wpb * 32, 0, st>>>(xp, ldx, yp, ldy, rows, c, gamma, beta, eps, apply_silu);
-    B200_CHECK_LAUNCH("layernorm_narrow");
-    return 0;
-  }
-#define LN_LAUNCH(MV)                                                                                              \
-  layernorm_kernel<MV><<<grid, wpb * 32, 0, st>>>(xp, ldx, yp, ldy, rows, c, gamma, beta, eps, fvec, ldf,          \
-                                                  rows_per_frame, xs, ldxs, apply_silu)
-  if (vecs <= 32) LN_LAUNCH(1);
-  else if (vecs <= 64) LN_LAUNCH(2);
-  else if (vecs <= 128) LN_LAUNCH(4);
-  else LN_LAUNCH(8);
-#undef LN_LAUNCH
-  B200_CHECK_LAUNCH("layernorm");
+  const int wpb = 8;
+  const int64_t rows_per_block = (int64_t)wpb * (32 / lpr);
+  const unsigned grid = (unsigned)((rows + rows_per_block - 1) / rows_per_block);
+  kernel<<<grid, wpb * 32, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      reinterpret_cast<const __nv_bfloat16*>(x), ldx, reinterpret_cast<__nv_bfloat16*>(y), ldy, rows, c, gamma, beta,
+      eps, fvec, ldf, rows_per_frame, reinterpret_cast<__nv_bfloat16*>(xsum), ldxs, apply_silu);
+  B200_CHECK_LAUNCH(name);
   return 0;
 }
 

@@ -18,7 +18,7 @@ GroupNorm (gn_stats + gn_apply)
   adds 2^-16 |pre-activation|.
 gn_stats_partials: the partials are small integers, so every sum is exact: torch.equal.
 
-LayerNorm (one warp, or LPR lanes, per row; fp32 two-pass statistics)
+LayerNorm (layernorm_kernel<LPR, V, VEC>: LPR lanes per row, V vectors per lane; fp32 two-pass statistics)
   mean and sum of squared deviations go through at most 8 * 8 per-lane adds and 5 shuffle levels: within 69 u
   (< 2^-17.9) of sum|v| and of the variance; rstd adds rsqrtf's 2 ulp; (v - mean) rstd g + b three roundings more.
       |y - ref| <= 2^-8 |ref| + 2^-16 (|xhat g| + rstd |g| mean|v|) + 2^-20 |b|      (xhat = (v - mean) rstd)
@@ -363,8 +363,9 @@ def test_gn_stats_partials_exact(cuda_dev, n_slots, C, ld, n):
 # LayerNorm
 # ---------------------------------------------------------------------------------------------------------------------
 LN_CASES = {
-    # name: rows, C, options.  Branches: layernorm5<8/16/32> (C 320/640/1280), narrow<4/8/16/32> (C <= 256 without
-    # fvec), generic with 1/2/4/8 vectors per lane (fvec, or C > 256, or misaligned gamma/beta/fvec)
+    # name: rows, C, options.  Branches, layernorm_kernel<lanes per row, vectors per lane, float4 parameters>: <8/16/32,
+    # 5, vec> (C 320/640/1280), narrow <4/8/16/32, 1, vec> (C <= 256 without fvec), generic <32, 1/2/4/8, scalar>
+    # (fvec, or C > 256, or misaligned gamma/beta/fvec)
     "ln5_320_fvec_xsum": (4097, 320, dict(fvec=1024, xsum=True)),
     "ln5_640_fvec_silu": (33, 640, dict(fvec=8, silu=True)),
     "ln5_1280_const": (33, 1280, dict(const=True)),
